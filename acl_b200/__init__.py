@@ -1,4 +1,4 @@
-"""acl_b200 -- B200-native (sm_100a) batched decompression of nfrechette/acl `compressed_tracks`.
+"""acl_b200 -- H100-native (sm_90a) batched decompression of nfrechette/acl `compressed_tracks`.
 
 The product is the C-ABI shared library `acl_b200/libaclb200.so` (sources in acl_b200/csrc/, interface in
 include/aclb200.h, C++ header shim in include/acl_b200/decompress.h). This Python package is only the thin

@@ -111,7 +111,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.3 (sm_100a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.3 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -171,9 +171,9 @@ extern "C"
 		context->device = device;
 		context->num_sms = prop.multiProcessorCount;
 		context->max_dynamic_smem = int(prop.sharedMemPerBlockOptin);
-		if (prop.major < 10 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess)
+		if (prop.major != 9 || prop.minor != 0 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess)
 		{
-			// the kernels are compiled for sm_100a only
+			// the kernels are compiled for sm_90a only, which runs on compute capability 9.0 and nothing else
 			delete context;
 			return ACLB200_ERR_NO_DEVICE;
 		}

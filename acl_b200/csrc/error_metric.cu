@@ -17,10 +17,10 @@
 // a handful of wavefronts per chunk). Object transforms live in shared memory as [component][bone] planes so that 32 lanes reading 32
 // different parents hit 32 different banks; a bone's local transform is parked in the slot its object transform will take. The
 // measurement itself (three shell points through both transforms) runs after the chunk's wavefronts with every lane busy, and the raw and
-// the lossy pose travel together as packed f32x2 values (FMUL2 / FFMA2).
+// the lossy pose travel together as f32x2 pairs (one scalar operation per lane on sm_90).
 //
-// Every float operation is the reference's, in its order, never fused (the library is built with --fmad=false, packed adds go through a
-// run-time 1.0f). The one exception is rtm::quat_normalize, whose SSE2 code starts from the CPU specific rsqrtss estimate
+// Every float operation is the reference's, in its order, never fused (the library is built with --fmad=false and uses the _rn
+// intrinsics). The one exception is rtm::quat_normalize, whose SSE2 code starts from the CPU specific rsqrtss estimate
 // (external/rtm/includes/rtm/quatf.h:917-953) and cannot be reproduced bit for bit by anyone: the IEEE 1 / sqrt stands in for it (the
 // tests' CPU restatement has both flavours; errors agree with the reference within 5e-5 on poses tens of units across,
 // tests/test_gpu_error_metric.py). The matrix metric never normalises: it is bit-identical to the reference itself.
@@ -83,10 +83,9 @@ namespace aclb200
 		};
 
 		// ---- the reference's float operations, spelled out so nothing can be contracted -------------------------------------------
-		// The measurement runs the SAME operation sequence on the raw and on the lossy pose: the two travel as one packed f32x2 value
-		// (x = raw, y = lossy) through mul.rn.f32x2 / fma.rn.f32x2, half the instructions of two scalar streams. ptxas contracts a packed
-		// mul + add into one FFMA2 even under --fmad=false, so the packed add is issued as fma(a, one, b) with `one` a run-time 1.0f
-		// (round(a * 1 + b) == round(a + b)), like pipeline.cu does. Signs: the reference xors sign masks into products and adds them;
+		// The measurement runs the SAME operation sequence on the raw and on the lossy pose: the two travel as one f32x2 pair
+		// (x = raw, y = lossy). sm_90 has no packed f32x2 pipe: each operation is one scalar __fmul_rn / __fadd_rn / __fsub_rn per lane,
+		// intrinsics that are never contracted into an FMA (`one` is not needed by them). Signs: the reference xors sign masks into products and adds them;
 		// -(p) + q == q - p, p + -(q) == p - q and -(p) + -(q) == -(p + q) hold exactly in IEEE arithmetic, so the sums below are written
 		// with subtractions and no negation (a packed operand has no free negate modifier).
 		template<class V> struct Fp;
@@ -105,9 +104,9 @@ namespace aclb200
 		template<> struct Fp<float2>
 		{
 			float one;
-			__device__ __forceinline__ float2 mul(float2 a, float2 b) const { return __fmul2_rn(a, b); }
-			__device__ __forceinline__ float2 add(float2 a, float2 b) const { return __ffma2_rn(a, make_float2(one, one), b); }
-			__device__ __forceinline__ float2 sub(float2 a, float2 b) const { return __ffma2_rn(b, make_float2(-one, -one), a); }
+			__device__ __forceinline__ float2 mul(float2 a, float2 b) const { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+			__device__ __forceinline__ float2 add(float2 a, float2 b) const { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+			__device__ __forceinline__ float2 sub(float2 a, float2 b) const { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
 			__device__ __forceinline__ float2 splat(float a) const { return make_float2(a, a); }
 			__device__ __forceinline__ float2 inv_sqrt(float2 a) const { return make_float2(__fdiv_rn(1.0f, __fsqrt_rn(a.x)), __fdiv_rn(1.0f, __fsqrt_rn(a.y))); }
 			__device__ __forceinline__ bool any_negative(float2 a, float2 b) const { return fminf(a.x, b.x) < 0.0f || fminf(a.y, b.y) < 0.0f; }

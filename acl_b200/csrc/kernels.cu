@@ -1,4 +1,4 @@
-// acl_b200/csrc/kernels.cu -- sm_100a kernels of the batched ACL decompression path.
+// acl_b200/csrc/kernels.cu -- sm_90a kernels of the batched ACL decompression path.
 //
 // One launch decodes `num_requests` (clip, sample_time) requests == that many
 //   context.seek(t, policy); context.decompress_tracks(writer);

@@ -199,7 +199,7 @@ def algorithmic_bytes_scalar(w) -> dict:
 MATH_DESCRIPTION = {
     "exact": "exact: every float bit-identical to the reference's SSE path (IEEE mul/add/sqrt/div in its order, never fused)",
     "fast": "fast: integer / format decode, translations and scales bit-exact; rotations use hardware sqrt / rsqrt and fused multiply-adds after "
-            "the exact W-reconstruction input, <= 1e-5 absolute vs the reference (north star gate; measured < 2e-6, tests/test_gpu_parity.py::test_fast_math_within_tolerance)",
+            "the exact W-reconstruction input, <= 1e-5 absolute vs the reference (north star gate, tests/test_gpu_parity.py::test_fast_math_within_tolerance)",
 }
 
 
@@ -323,7 +323,7 @@ def bounded_sample(w, threads: int, seconds: float = 4.0) -> int:
 def bind_to_gpu_numa_node(local_rank: int) -> dict:
     """Pins this rank's host threads to the CPUs of its GPU's NUMA node BEFORE any pinned host buffer is allocated (first touch then
     places the pages next to the GPU's PCIe root). Without it the ranks of an 8 GPU box share one node's memory controllers and
-    the D2H copies of the e2e path collapse (round 1: 0.54 G bone-poses/s per GPU at N=8 against 1.32 alone)."""
+    the D2H copies of the e2e path collapse."""
     info = {"numa_node": None, "cpus": None}
     try:
         import pynvml
@@ -355,7 +355,7 @@ def workload_config(args, w, world: int, num_requests: int, pose_bytes: int, blo
     is_transform = w["kind"] == "transform"
     return {"workload": w["description"], "clips": "distinct" if w["distinct"] else "replicated", "clips_per_gpu": w["num_clips"],
             "requests_per_step_per_gpu": num_requests, "bones": w["num_tracks"], "layout": args.layout,
-            "l2": f"inputs larger than L2: {blob_bytes / 1e6:.0f} MB compressed + {num_requests * pose_bytes / 1e6:.0f} MB of poses per step vs 126 MB L2",
+            "l2": f"inputs larger than L2: {blob_bytes / 1e6:.0f} MB compressed + {num_requests * pose_bytes / 1e6:.0f} MB of poses per step vs 50 MB L2 (H100)",
             "math": MATH_DESCRIPTION[args.math if is_transform else "exact"], "parallelism": f"clip-sharded x{world}, no data-path collective"}
 
 
@@ -409,7 +409,12 @@ def main() -> None:
     ap.add_argument("--gather", action="store_true", help="N > 1: also time decode + NCCL all-gather of the poses (SURVEY 8e, optional consumer-side gather)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the extra blocks (other workloads at N = 1, the routed C5 job at N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the poses the last timed step decoded (a fixed, seeded sample of the requests) as "
+                         "DIR/*.npy (bench_outputs/ in the repository is git-ignored)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -499,6 +504,8 @@ def main() -> None:
     launches_before = ctx.launch_count
     rank_ms, kernel_ms = time_launches(torch, launch, stream, args.steps, args.warmup, barrier, sampler)
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, torch, d_out, num_requests, pose_bytes, "" if world == 1 else f"_rank{rank}")
     gpu_launches = ctx.launch_count - launches_before - args.warmup
     elapsed_ms = reducer.max(rank_ms)                                   # slowest rank
     value = reducer.sum(units_per_step * args.steps) / (elapsed_ms * 1e-3)   # every rank's units
@@ -540,7 +547,7 @@ def main() -> None:
         h_out = torch.empty(num_requests * pose_bytes, dtype=torch.uint8).pin_memory()
         req_np = h_requests.numpy().view(ab.api.REQUEST_DTYPE)
         out_np = h_out.numpy()
-        e2e_steps = max(args.steps, 2)
+        e2e_steps = args.steps
         for _ in range(2):
             ctx.decompress_tracks_host(clipset, req_np, options, out_np)     # warm-up (allocates the device scratch)
         barrier()
@@ -572,7 +579,7 @@ def main() -> None:
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
     written_per_step = alg["out_bytes"] * bone_bytes // 40 if is_transform else alg["out_bytes"]
     achieved = (alg["in_bytes"] + alg["out_bytes"]) / (kernel_ms * 1e-3) / 1e9
     traffic, traffic_source = measured_traffic(args.workload)
@@ -629,6 +636,23 @@ def main() -> None:
     print(json.dumps(result))
     if distributed:
         dist.destroy_process_group()
+
+
+DUMP_BYTES = 48 << 20       # the dumped sample stays well under 64 MB
+
+
+def dump_outputs(directory: str, torch, d_out, num_requests: int, pose_bytes: int, suffix: str) -> None:
+    """Writes the pose rows of a fixed, seeded sample of the requests as <directory>/poses<suffix>.npy (float32, one row of
+    bones x floats per bone for each sampled request, as the caller's output buffer holds it) and their request indices as
+    request_index<suffix>.npy (float64)."""
+    os.makedirs(directory, exist_ok=True)
+    count = min(num_requests, DUMP_BYTES // pose_bytes)
+    index = np.sort(np.random.default_rng(0).choice(num_requests, size=count, replace=False))
+    rows = d_out.view(num_requests, pose_bytes).index_select(0, torch.from_numpy(index).to(d_out.device))
+    poses = rows.cpu().numpy().view(np.float32).reshape(count, -1)
+    np.save(os.path.join(directory, f"poses{suffix}.npy"), poses)
+    np.save(os.path.join(directory, f"request_index{suffix}.npy"), index.astype(np.float64))
+    log(f"[bench] wrote {count} of {num_requests} pose rows to {directory}")
 
 
 def sample_single_thread(w, blobs) -> float:

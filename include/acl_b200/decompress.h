@@ -30,7 +30,7 @@
 // compatibility and for tests. Throughput comes from batch_context / batch_decompressor below: upload the clips once, decode
 // thousands of (clip, sample_time) requests per launch into device memory.
 //
-// Nothing here decodes on the CPU: without the library or without a B200 every call fails with a status, never silently.
+// Nothing here decodes on the CPU: without the library or without an H100 every call fails with a status, never silently.
 #pragma once
 
 #include "../aclb200.h"

@@ -1,4 +1,4 @@
-/* include/aclb200.h -- C ABI of libaclb200.so: batched, B200-native (sm_100a) decompression of
+/* include/aclb200.h -- C ABI of libaclb200.so: batched, H100-native (sm_90a) decompression of
  * nfrechette/acl `compressed_tracks` blobs.
  *
  * ACL (reference @ 0f855f0) has no FFI layer of its own: its "operator API" for this path is the
@@ -70,8 +70,8 @@ enum
 	ACLB200_MATH_EXACT = 0,		/* IEEE-754 mul/add/sqrt/div in the reference's operation order, never fused: bit-identical
 								 * to the reference's SSE2/AVX/scalar builds for decompress_tracks */
 	ACLB200_MATH_FAST = 1		/* decompress_tracks on variable bit rate rotations: x, y, z and the W reconstruction input stay exact,
-								 * then hardware sqrt / rsqrt and fused multiply-adds: rotations <= 1e-5 absolute from EXACT (measured
-								 * < 2e-6, including W ~ 0), translations / scales / every other path unchanged (bit-exact) */
+								 * then hardware sqrt / rsqrt and fused multiply-adds: rotations <= 1e-5 absolute from EXACT
+								 * (including W ~ 0), translations / scales / every other path unchanged (bit-exact) */
 };
 
 typedef struct aclb200_context aclb200_context;

@@ -41,6 +41,17 @@ def main() -> None:
                             error=np.float32(r["error"]), sample_time=np.float32(r["sample_time"]), rounding=np.uint32(r["rounding"]),
                             sample_rate=np.float32(r["sample_rate"]), duration=np.float32(r["duration"]))
         print("scalar", name, r["index"], r["error"], r["sample_time"])
+    write_matrix_golden()
+
+
+def write_matrix_golden() -> None:
+    """tests/golden/*.matrix_error.npz: qvvf_matrix3x4f_transform_error_metric over the same raw poses. That metric has no CPU specific
+    step, so these numbers are the reference's on any machine and the tests compare them bit for bit."""
+    for name in TRANSFORM:
+        m = ref.transform_error_matrix(clips.TRANSFORM_SPECS[name], clips.load_blob(name))
+        np.savez_compressed(clips.golden_path(name, "matrix_error.npz"), errors=m["errors"], index=np.uint32(m["index"]),
+                            error=np.float32(m["error"]), sample_time=np.float32(m["sample_time"]))
+        print("matrix", name, m["index"], m["error"], m["sample_time"])
 
 
 if __name__ == "__main__":

@@ -180,6 +180,19 @@ def test_port_matches_golden_errors(oracle_port, name):
         assert g["errors"][sample, got.index] >= float(g["error"]) - 2 * ERROR_TOLERANCE, (name, mode)
 
 
+@pytest.mark.parametrize("name", GOLDEN_TRANSFORM)
+def test_port_matrix_metric_matches_golden(oracle_port, name):
+    """The reference's qvvf_matrix3x4f_transform_error_metric numbers committed with the clip: no CPU specific step, bit for bit."""
+    blob = clips.load_blob(name)
+    g = np.load(clips.golden_path(name, "error.npz"))
+    m = np.load(clips.golden_path(name, "matrix_error.npz"))
+    lossy = lossy_poses_from_port(blob, 1, g["raw_poses"].shape[0], float(g["sample_rate"]), float(g["duration"]), int(g["rounding"]))
+    got, errors, _ = oracle_port.transform_track_error(g["raw_poses"], lossy, float(g["sample_rate"]), float(g["duration"]), g["parents"],
+                                                       g["shell_distances"], P.NORMALIZE_IEEE, metric=1)
+    assert clips.bit_equal(errors, m["errors"]), name
+    assert (got.index, np.float32(got.error), np.float32(got.sample_time)) == (int(m["index"]), np.float32(m["error"]), np.float32(m["sample_time"])), name
+
+
 def lossy_scalar_from_port(blob, num_samples, sample_rate, duration, rounding):
     settings = P.settings_for_kind(0)
     rows = []

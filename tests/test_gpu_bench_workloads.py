@@ -5,7 +5,8 @@ debug_track_writer style pose, oracle/ref_tool.cpp aclref_bench_transform / aclr
 Mirrors what the reference's own validation walks (tools/acl_compressor/sources/validate_tracks.cpp:92-260,328-511).
 
 Bar: ACLB200_MATH_EXACT bit-identical on every defined lane; ACLB200_MATH_FAST rotations <= 1e-5 absolute, translations and
-scales bit-identical. Needs the compiled reference (it travels to the GPU box prebuilt); skipped without it.
+scales bit-identical. The exhaustive tests need the compiled reference and are skipped without it; a fixed sample of the
+same clips and requests is compared with the reference's stored output (tests/golden/bench_workloads.npz) everywhere.
 """
 import numpy as np
 import pytest
@@ -87,6 +88,39 @@ def test_bench_workload_every_request_vs_reference(env, name, slice_requests):
     clipset.release()
 
 
+@pytest.mark.parametrize("name", ["c2", "c5"])
+def test_bench_workload_sample_vs_stored_reference(name):
+    """A fixed sample of the benchmarked clips and requests (tests/golden/make_bench_golden.py) against what the reference decoded for
+    them, stored with the clips: the same bar as above without the compiled reference. The sample must also still be what bench.py
+    builds when the reference compressor is at hand."""
+    import torch
+    import acl_b200 as ab
+    from oracle import ref
+    golden = np.load(clips.golden_path("bench_workloads", "npz"))
+    sizes = golden[f"{name}_sizes"]
+    ends = np.cumsum(sizes.astype(np.int64))
+    blobs = [ref.aligned_blob(golden[f"{name}_blobs"][end - size:end]) for size, end in zip(sizes, ends)]
+    req_clip, req_time, want = golden[f"{name}_req_clip"], golden[f"{name}_req_time"], golden[f"{name}_want"]
+    if ref.available():
+        import bench
+        w = bench.make_workload(name, 0, len(blobs))
+        assert np.array_equal(np.concatenate([w["buffer"][int(o):int(o) + int(s)] for o, s in zip(w["offsets"], w["sizes"])]), golden[f"{name}_blobs"])
+    ctx = ab.Context(0)
+    clipset = ctx.upload(blobs, check_hash=True)
+    n = len(req_clip)
+    d_requests = torch.from_numpy(ab.make_requests(req_clip, req_time).view(np.uint8)).cuda()
+    got = {}
+    for mode in (ab.MATH_EXACT, ab.MATH_FAST):
+        d_out = torch.full((n, clipset.max_tracks, 12), float("nan"), dtype=torch.float32, device="cuda")
+        ctx.decompress_tracks(clipset, d_requests, n, ab.Options(output_layout=ab.LAYOUT_QVV48, math_mode=mode), d_out)
+        torch.cuda.synchronize()
+        got[mode] = d_out.cpu().numpy()[:, :, LANES]
+    assert clips.bit_equal(got[ab.MATH_EXACT], want)
+    assert clips.bit_equal(got[ab.MATH_FAST][:, :, 4:], want[:, :, 4:])
+    assert float(np.abs(got[ab.MATH_FAST][:, :, :4] - want[:, :, :4]).max()) <= FAST_MATH_TOLERANCE
+    clipset.release()
+
+
 def test_bench_workload_c4_every_request_vs_reference(env):
     """C4: scalar float1f 4096 tracks x 1024 samples replicated x64, the 65 536 requests bench.py times."""
     import bench
@@ -113,7 +147,10 @@ def test_bench_workload_c4_every_request_vs_reference(env):
 # v02_00_00 clips: the raw bit rate marker is 32 instead of 31 (animated_track_cache.transform.h:523), scalar tracks use the 19 entry
 # bit rate table (decompression.scalar.h:259-263), the wrap flag does not exist (compressed_tracks.impl.h:127-134). The compressor
 # here only writes the latest version: the fixtures are golden blobs re-labelled on the host (version field, markers / table
-# indices re-mapped so that the payload means the same, hash recomputed) and decoded by the unmodified reference.
+# indices re-mapped so that the payload means the same, hash recomputed) and decoded by the unmodified reference. A scalar track
+# whose bit rate the v02_00_00 table lacks (1, 2 or 20-23 bits) is re-quantized to the nearest rate it has (3 or 19 bits) and the
+# key frame stream repacked: the payload then means something slightly different, which is fine, because the reference decodes the
+# very same re-labelled clip.
 # ------------------------------------------------------------------------------------------------------------------
 def _fnv1a32(data: np.ndarray) -> int:
     acc = 2166136261
@@ -124,7 +161,7 @@ def _fnv1a32(data: np.ndarray) -> int:
 
 def _as_version_7(blob: np.ndarray):
     """Returns (re-labelled blob, number of raw / re-mapped entries), or None when the clip cannot be expressed in v02_00_00."""
-    b = blob.copy()
+    b = blob.copy() if int(blob[15]) == 12 else _requantize_scalar_for_version_7(blob)
     u32 = lambda off: int(b[off:off + 4].view(np.uint32)[0])
     size = u32(0)
     track_type, misc = int(b[15]), u32(28)
@@ -140,19 +177,53 @@ def _as_version_7(blob: np.ndarray):
             touched += int((fmt == 31).sum())
             fmt[fmt == 31] = 32
     else:
-        v10 = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 32]
-        v7 = [0, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 32]
+        v10, v7 = V10_SCALAR_BITS, V7_SCALAR_BITS
         num_tracks = u32(16)
         meta = 32 + u32(32 + 4)
         rates = b[meta:meta + num_tracks]
-        bits = [v10[r] for r in rates]
-        if any(x not in v7 for x in bits):
-            return None
-        rates[:] = [v7.index(x) for x in bits]
+        rates[:] = [v7.index(v10[r]) for r in rates]
         touched = num_tracks
     b[12:14] = np.array([7], dtype=np.uint16).view(np.uint8)
     b[4:8] = np.array([_fnv1a32(b[8:size])], dtype=np.uint32).view(np.uint8)
     return b, touched
+
+
+V10_SCALAR_BITS = [0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 32]
+V7_SCALAR_BITS = [0, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 32]
+
+
+def _requantize_scalar_for_version_7(blob: np.ndarray) -> np.ndarray:
+    """A copy of a (latest version) scalar clip whose variable bit rates all exist in the v02_00_00 table: a 1 or 2 bit track becomes
+    3 bits, a 20-23 bit track 19 bits (values shifted by the difference). The key frame stream is the clip's last section: frames of
+    num_bits_per_frame bits, tracks in order, each animated track's components MSB first (decompression.scalar.h:212-481)."""
+    u32 = lambda off: int(blob[off:off + 4].view(np.uint32)[0])
+    size, num_tracks, num_samples = u32(0), u32(16), u32(20)
+    components = int(blob[15]) + 1 if int(blob[15]) <= 3 else 4
+    bits_per_frame, meta, animated = u32(32), 32 + u32(36), 32 + u32(48)
+    old_bits = [V10_SCALAR_BITS[r] for r in blob[meta:meta + num_tracks]]
+    new_bits = [x if x in V7_SCALAR_BITS else (3 if x < 3 else 19) for x in old_bits]
+    if new_bits == old_bits:
+        return blob.copy()
+    old_bytes = (num_samples * bits_per_frame + 7) // 8
+    stream = np.unpackbits(blob[animated:animated + old_bytes])
+    new_bits_per_frame = components * sum(new_bits)
+    out_stream = np.zeros(num_samples * new_bits_per_frame, dtype=np.uint8)
+    weights = lambda n: (1 << np.arange(n - 1, -1, -1, dtype=np.uint64))
+    for frame in range(num_samples):
+        src, dst = frame * bits_per_frame, frame * new_bits_per_frame
+        for old, new in zip(old_bits, new_bits):
+            for _ in range(components if old else 0):
+                value = int(stream[src:src + old].astype(np.uint64) @ weights(old))
+                value = value >> (old - new) if old > new else value << (new - old)
+                out_stream[dst:dst + new] = (value >> np.arange(new - 1, -1, -1)) & 1
+                src, dst = src + old, dst + new
+    tail = size - animated - old_bytes
+    packed = np.packbits(out_stream)
+    b = np.concatenate([blob[:animated], packed, np.zeros(tail, np.uint8)])
+    b[0:4] = np.array([b.size], dtype=np.uint32).view(np.uint8)
+    b[32:36] = np.array([new_bits_per_frame], dtype=np.uint32).view(np.uint8)
+    b[meta:meta + num_tracks] = [V10_SCALAR_BITS.index(x) for x in new_bits]
+    return b
 
 
 @pytest.mark.parametrize("name", ["noisy_raw", "mixed_scale", "c1_30bones", "full_formats"])
@@ -183,12 +254,11 @@ def test_v02_00_00_transform_clip_vs_reference(env, name):
     clipset.release()
 
 
-@pytest.mark.parametrize("name", ["float1", "float3", "vector4"])
+@pytest.mark.parametrize("name", ["float1", "float2", "float3", "vector4"])
 def test_v02_00_00_scalar_clip_vs_reference(env, name):
     torch, ab, ref, ctx = env["torch"], env["ab"], env["ref"], env["ctx"]
     made = _as_version_7(clips.load_blob(name))
-    if made is None:
-        pytest.skip("this clip uses bit rates the v02_00_00 table does not have")
+    assert made is not None
     blob = ref.aligned_blob(made[0])
     assert ref.lib().aclref_is_valid(blob.ctypes.data, 1) == 0
     clipset = ctx.upload([blob], check_hash=True)

@@ -237,20 +237,28 @@ def test_compression_error_with_negative_scales(gpu, name, negative_scale_pct):
     clipset.release()
 
 
-@pytest.mark.parametrize("name", ["c1_30bones", "c2_100bones", "mixed_scale", "stripped_single", "paragon_like", "ragged_17", "one_bone", "mirrored"])
+@pytest.mark.parametrize("name", ["c1_30bones", "c2_100bones", "mixed_scale", "stripped_single", "paragon_like", "ragged_17", "one_bone", "mirrored",
+                                  "single_segment", "two_samples"])
 def test_matrix_metric_matches_the_reference_exactly(gpu, name):
     """ACLB200_METRIC_QVVF_MATRIX3X4F == qvvf_matrix3x4f_transform_error_metric: no CPU specific step, so the device must give the
     reference's numbers bit for bit (every per bone error, the worst track, its error and sample time); measured next to a job of the
-    same clip with the default metric in one call."""
+    same clip with the default metric in one call. Without the compiled reference its committed numbers stand in
+    (tests/golden/*.matrix_error.npz, machine independent: the metric has no CPU specific step)."""
     from oracle import ref
-    if not ref.available():
-        pytest.skip("needs oracle/_ref/libaclref.so")
     ab = gpu["ab"]
     spec = mirrored_spec("mixed_scale", 30) if name == "mirrored" else clips.TRANSFORM_SPECS[name]
-    blob = ref.compress_transform(spec) if name == "mirrored" else clips.load_blob(name)
+    if ref.available():
+        blob = ref.compress_transform(spec) if name == "mirrored" else clips.load_blob(name)
+        r = ref.transform_error(spec, blob, 1)
+        m = ref.transform_error_matrix(spec, blob)
+    elif name in GOLDEN_TRANSFORM:
+        blob = clips.load_blob(name)
+        r = _reference_case(name, 1)
+        g = np.load(clips.golden_path(name, "matrix_error.npz"))
+        m = dict(errors=g["errors"], index=int(g["index"]), error=float(g["error"]), sample_time=float(g["sample_time"]))
+    else:
+        pytest.skip("needs oracle/_ref/libaclref.so")
     clipset = gpu["ctx"].upload([blob])
-    r = ref.transform_error(spec, blob, 1)
-    m = ref.transform_error_matrix(spec, blob)
     common = dict(clip=0, num_samples=spec.num_samples, sample_rate=r["sample_rate"], duration=r["duration"], num_tracks=spec.num_tracks)
     jobs = _jobs(gpu, [dict(common), dict(common, error_metric=ab.api.METRIC_QVVF_MATRIX3X4F)])
     got, matrix = _measure(gpu, clipset, jobs, r["raw_poses"], r["parents"], r["shell_distances"], _options(gpu, 1))

@@ -1,4 +1,4 @@
-// Development experiment: what do partial-sector global stores of 40 byte bones cost in DRAM traffic on B200?
+// Development experiment: what do partial-sector global stores of 40 byte bones cost in DRAM traffic on an H100?
 // mode 0: each thread writes only the 16 byte rotation of its bone (28 of 40 bytes untouched)
 // mode 1: each thread writes rotation (16 B), translation (12 B), scale (12 B) of its bone back to back
 // mode 2: like 1, but translation+scale are written by a different warp of the block, one "chunk" later
@@ -55,9 +55,9 @@ int main()
 	for (int mode = 0; mode < 3; ++mode)
 	{
 		cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
-		k<<<148 * 8, 256>>>(out, bones, mode);
+		k<<<132 * 8, 256>>>(out, bones, mode);
 		cudaEventRecord(a);
-		k<<<148 * 8, 256>>>(out, bones, mode);
+		k<<<132 * 8, 256>>>(out, bones, mode);
 		cudaEventRecord(b); cudaEventSynchronize(b);
 		float ms; cudaEventElapsedTime(&ms, a, b);
 		printf("mode %d: %.3f ms (%.1f GB/s of 2.4 GB)\n", mode, ms, 2.4 / ms * 1000);

@@ -1,6 +1,6 @@
-// Development experiment: how fast can B200 drain 2.4 GB of pose rows through 1-D TMA bulk stores (cp.async.bulk shared -> global),
+// Development experiment: how fast can an H100 drain 2.4 GB of pose rows through 1-D TMA bulk stores (cp.async.bulk shared -> global),
 // nothing else going on? The floor of the pipeline kernel's output side.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tma_store_floor tma_store_floor.cu && ./tma_store_floor
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tma_store_floor tma_store_floor.cu && ./tma_store_floor
 // Each block owns a contiguous range of the output and loops: (optionally touch the chunk in shared memory) -> fence -> one bulk store
 // of `chunk` bytes -> commit; a stage is reused once wait_group.read says the copy has read it.
 #include <cstdio>
@@ -53,7 +53,7 @@ float run(uint8_t* out, uint64_t total, uint32_t chunk, int blocks_per_sm, int t
 	for (int r = 0; r < 4; ++r)
 	{
 		cudaEventRecord(a);
-		store_kernel<STAGES><<<148 * blocks_per_sm, 128, STAGES * chunk>>>(out, total, chunk, touch);
+		store_kernel<STAGES><<<132 * blocks_per_sm, 128, STAGES * chunk>>>(out, total, chunk, touch);
 		cudaEventRecord(b); cudaEventSynchronize(b);
 		float ms; cudaEventElapsedTime(&ms, a, b);
 		if (r > 0 && ms < best) best = ms;
@@ -72,7 +72,7 @@ int main()
 		for (int r = 0; r < 3; ++r)
 		{
 			cudaEventRecord(a);
-			plain_store_kernel<<<148 * 8, 256>>>(reinterpret_cast<float4*>(out), total / 16);
+			plain_store_kernel<<<132 * 8, 256>>>(reinterpret_cast<float4*>(out), total / 16);
 			cudaEventRecord(b); cudaEventSynchronize(b);
 			float ms; cudaEventElapsedTime(&ms, a, b);
 			if (r == 2) printf("plain coalesced 16 B stores: %.3f ms  %.0f GB/s\n", ms, total / ms / 1e6);

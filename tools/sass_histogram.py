@@ -1,6 +1,6 @@
-"""SASS opcode histogram of the library's kernels (what proves a Blackwell-native, non-contraction kernel: UBLKCP / UBLKPF = 1-D bulk
-TMA, SYNCS = mbarrier, FMUL2 / FFMA2 = packed f32x2; no HMMA / UTC*MMA expected: there is no contraction on this path).
-   python tools/sass_histogram.py acl_b200/libaclb200.so > profiles/r02_sass_histogram.txt"""
+"""SASS opcode histogram of the library's kernels (what shows a Hopper-native, non-contraction kernel: UBLKCP / UBLKPF = 1-D bulk
+TMA, SYNCS = mbarrier; no HMMA / HGMMA expected: there is no contraction on this path).
+   python tools/sass_histogram.py acl_b200/libaclb200.so > sass_histogram.txt"""
 import collections, re, subprocess, sys
 lib = sys.argv[1]
 txt = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True).stdout
@@ -20,5 +20,5 @@ for block in txt.split("Function : ")[1:]:
         print(f"\n{short[:100]}: {sum(ops.values())} instructions")
         print("  " + ", ".join(f"{k} {v}" for k, v in ops.most_common(28)))
 print("\nwhole library:", sum(total.values()), "instructions")
-for key in ("UBLKCP", "UBLKPF", "SYNCS", "FMUL2", "FFMA2", "UTMACMDFLUSH", "ATOMS", "HMMA", "UTCHMMA", "LDGSTS"):
+for key in ("UBLKCP", "UBLKPF", "SYNCS", "UTMACMDFLUSH", "ATOMS", "HMMA", "HGMMA", "LDGSTS"):
     print(f"  {key:14s} {total.get(key, 0)}")
