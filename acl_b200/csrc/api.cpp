@@ -1,7 +1,6 @@
 // acl_b200/csrc/api.cpp -- the extern "C" surface declared in include/aclb200.h.
 #include "context.h"
 
-#include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <new>
@@ -273,10 +272,7 @@ extern "C"
 		const bool any_skipped = options->default_rotation_mode == ACLB200_DEFAULT_SKIPPED || options->default_translation_mode == ACLB200_DEFAULT_SKIPPED
 			|| options->default_scale_mode == ACLB200_DEFAULT_SKIPPED;
 		const bool any_masked = (options->skip_mask & 7u) != 0 || options->d_skip_track_mask != nullptr;
-		// ACLB200_PIPELINE=0 sends everything through the plain kernels (tuning / A-B measurements)
-		static const char* const override_pipeline = std::getenv("ACLB200_PIPELINE");
-		const bool pipeline_allowed = override_pipeline == nullptr || override_pipeline[0] != '0';
-		if (pipeline_allowed && !any_skipped && !any_masked && clipset->max_key_frame_bytes != 0)
+		if (!any_skipped && !any_masked && clipset->max_key_frame_bytes != 0)
 		{
 			DecodeParams pipeline_params = params;
 			if (plan_pipeline(pipeline_params, clipset->max_key_frame_bytes, context->max_dynamic_smem, context->num_sms))

@@ -112,13 +112,11 @@ namespace aclb200
 		uint32_t out_bulk;					// pipeline: every pose row is 16 byte granular, rows leave shared memory as TMA bulk stores
 		uint32_t grid_blocks;				// pipeline: persistent grid size
 		uint32_t smem_stage_size;			// pipeline: bytes of one stage (key frame windows + poses)
-		uint32_t contiguous_batches;		// pipeline: every block takes one contiguous range of batches (else batches strided by the grid)
 		uint32_t hot_slot_bytes;			// pipeline: bytes of one slot of the ReqHot ring (records + group words)
 		uint32_t smem_tag_offset;			// pipeline: base row tags (which clip's base pose each pose row holds)
 		unsigned long long* trace;			// pipeline, ACLB200_PIPE_TRACE builds: clock stamps per (block, iteration), see aclb200_debug_set_trace
 		uint32_t trace_blocks;
 		uint32_t trace_iterations;
-		float    one;						// 1.0f the compiler cannot see (keeps f32x2 mul + add unfused, see pipeline.cu)
 		const uint8_t* base_poses;			// pipeline: base pose row per clip (nullptr: phase A runs in the kernel)
 		uint32_t base_stride;
 		uint8_t* out;

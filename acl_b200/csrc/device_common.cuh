@@ -27,15 +27,14 @@ namespace aclb200
 		// ---- f32x2 pair arithmetic ----
 		// The x and y lanes of a pair run the same operation sequence. sm_90 has no packed f32x2 pipe, so each helper issues one scalar
 		// IEEE operation per lane; __fmul_rn / __fadd_rn / __fsub_rn are never contracted into an FMA, which keeps every result
-		// bit-identical to the reference's separate mul and add. `one` (DecodeParams::one, a run-time 1.0f) is not needed by the
-		// scalar form and is ignored.
+		// bit-identical to the reference's separate mul and add.
 		__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(fmul(a.x, b.x), fmul(a.y, b.y)); }
 		__device__ __forceinline__ float2 mul2(float2 a, float b) { return make_float2(fmul(a.x, b), fmul(a.y, b)); }
-		__device__ __forceinline__ float2 add2(float2 a, float2 b, float) { return make_float2(fadd(a.x, b.x), fadd(a.y, b.y)); }		// a + b
-		__device__ __forceinline__ float2 sub2(float2 a, float2 b, float) { return make_float2(fsub(a.x, b.x), fsub(a.y, b.y)); }		// a - b
-		__device__ __forceinline__ float2 muladd2(float2 a, float2 b, float2 c, float) { return make_float2(fmuladd(a.x, b.x, c.x), fmuladd(a.y, b.y, c.y)); }
-		__device__ __forceinline__ float2 muladd2(float2 a, float b, float c, float) { return make_float2(fmuladd(a.x, b, c), fmuladd(a.y, b, c)); }
-		__device__ __forceinline__ float2 negmulsub2(float2 a, float2 b, float2 c, float) { return make_float2(fnegmulsub(a.x, b.x, c.x), fnegmulsub(a.y, b.y, c.y)); }
+		__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(fadd(a.x, b.x), fadd(a.y, b.y)); }		// a + b
+		__device__ __forceinline__ float2 sub2(float2 a, float2 b) { return make_float2(fsub(a.x, b.x), fsub(a.y, b.y)); }		// a - b
+		__device__ __forceinline__ float2 muladd2(float2 a, float2 b, float2 c) { return make_float2(fmuladd(a.x, b.x, c.x), fmuladd(a.y, b.y, c.y)); }
+		__device__ __forceinline__ float2 muladd2(float2 a, float b, float c) { return make_float2(fmuladd(a.x, b, c), fmuladd(a.y, b, c)); }
+		__device__ __forceinline__ float2 negmulsub2(float2 a, float2 b, float2 c) { return make_float2(fnegmulsub(a.x, b.x, c.x), fnegmulsub(a.y, b.y, c.y)); }
 
 		// ---------------------------------------------------------------------------------------------------
 		// TMA bulk copy + mbarrier (PTX ISA: cp.async.bulk, mbarrier)

@@ -79,20 +79,17 @@ namespace aclb200
 			uint32_t error_stride;			// floats per row of the matrix
 			uint32_t plane_stride;			// floats per [component] plane of a warp's object transforms
 			uint32_t components;			// scalar clips
-			float    one;					// 1.0f the compiler cannot see (keeps the packed mul + add unfused)
 		};
 
 		// ---- the reference's float operations, spelled out so nothing can be contracted -------------------------------------------
 		// The measurement runs the SAME operation sequence on the raw and on the lossy pose: the two travel as one f32x2 pair
-		// (x = raw, y = lossy). sm_90 has no packed f32x2 pipe: each operation is one scalar __fmul_rn / __fadd_rn / __fsub_rn per lane,
-		// intrinsics that are never contracted into an FMA (`one` is not needed by them). Signs: the reference xors sign masks into products and adds them;
-		// -(p) + q == q - p, p + -(q) == p - q and -(p) + -(q) == -(p + q) hold exactly in IEEE arithmetic, so the sums below are written
-		// with subtractions and no negation (a packed operand has no free negate modifier).
+		// (x = raw, y = lossy). Each operation is one scalar __fmul_rn / __fadd_rn / __fsub_rn per lane, intrinsics that are never
+		// contracted into an FMA. Signs: the reference xors sign masks into products and adds them; -(p) + q == q - p, p + -(q) == p - q
+		// and -(p) + -(q) == -(p + q) hold exactly in IEEE arithmetic, so the sums below are written with subtractions and no negation.
 		template<class V> struct Fp;
 
 		template<> struct Fp<float>
 		{
-			float one;
 			__device__ __forceinline__ float mul(float a, float b) const { return __fmul_rn(a, b); }
 			__device__ __forceinline__ float add(float a, float b) const { return __fadd_rn(a, b); }
 			__device__ __forceinline__ float sub(float a, float b) const { return __fsub_rn(a, b); }
@@ -103,7 +100,6 @@ namespace aclb200
 
 		template<> struct Fp<float2>
 		{
-			float one;
 			__device__ __forceinline__ float2 mul(float2 a, float2 b) const { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 			__device__ __forceinline__ float2 add(float2 a, float2 b) const { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 			__device__ __forceinline__ float2 sub(float2 a, float2 b) const { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
@@ -166,7 +162,7 @@ namespace aclb200
 
 		__device__ __forceinline__ Matrix3x4 matrix_from_qvv(const Qvv<float>& q)
 		{
-			const Fp<float> fp{ 1.0f };
+			const Fp<float> fp{};
 			const float x2 = fp.add(q.rotation.x, q.rotation.x), y2 = fp.add(q.rotation.y, q.rotation.y), z2 = fp.add(q.rotation.z, q.rotation.z);
 			const float xx = fp.mul(q.rotation.x, x2), xy = fp.mul(q.rotation.x, y2), xz = fp.mul(q.rotation.x, z2);
 			const float yy = fp.mul(q.rotation.y, y2), yz = fp.mul(q.rotation.y, z2), zz = fp.mul(q.rotation.z, z2);
@@ -181,7 +177,7 @@ namespace aclb200
 
 		__device__ __noinline__ void qvv_mul_negative_scale(const Qvv<float>* lhs_in, const Qvv<float>* rhs_in, Qvv<float>* out)
 		{
-			const Fp<float> fp{ 1.0f };
+			const Fp<float> fp{};
 			const Qvv<float> lhs = *lhs_in, rhs = *rhs_in;
 			const Matrix3x4 l = matrix_from_qvv(lhs), r = matrix_from_qvv(rhs);
 			float m[4][3];
@@ -550,7 +546,7 @@ namespace aclb200
 		// rtm::qvv_mul on one stream, whichever branch it takes
 		__device__ __forceinline__ Qvv<float> qvv_mul_any(const Qvv<float>& lhs, const Qvv<float>& rhs)
 		{
-			const Fp<float> fp{ 1.0f };
+			const Fp<float> fp{};
 			if (!takes_negative_branch(fp, lhs.scale, rhs.scale))
 				return qvv_mul_positive(fp, lhs, rhs);
 			Qvv<float> out;
@@ -562,7 +558,7 @@ namespace aclb200
 		template<class V>
 		__device__ __noinline__ void object_transform_slow(V* planes, uint32_t plane_stride, uint32_t bone, uint32_t parent)
 		{
-			const Fp<float> fp{ 1.0f };
+			const Fp<float> fp{};
 			for (int stream = 0; stream < Streams<V>::count; ++stream)
 			{
 				Qvv<float> out = qvv_mul_any(read_stream(planes, plane_stride, bone, stream), read_stream(planes, plane_stride, parent, stream));
@@ -628,7 +624,6 @@ namespace aclb200
 			const uint32_t* parent_indices;
 			uint32_t plane_stride;
 			uint32_t* flags;				// [1]
-			float    one;
 		};
 
 		// METRIC (MODE 0 only): 0 = qvvf_transform_error_metric, 1 = qvvf_matrix3x4f_transform_error_metric
@@ -644,8 +639,7 @@ namespace aclb200
 			constexpr uint32_t k_components = METRIC == 1 ? 12u : k_object_components;
 			V* planes = reinterpret_cast<V*>(object_plane_bytes) + size_t(warp) * k_components * plane_stride;
 			const uint64_t num_poses = MODE == 0 ? uint64_t(ep.num_poses) : op.num_poses;
-			Fp<V> fp;
-			fp.one = MODE == 0 ? ep.one : op.one;
+			const Fp<V> fp{};
 
 			for (uint64_t pose = uint64_t(blockIdx.x) * warps_per_block + warp; pose < num_poses; pose += uint64_t(gridDim.x) * warps_per_block)
 			{
@@ -960,7 +954,6 @@ extern "C"
 		op.parent_indices = d_parent_indices;
 		op.plane_stride = plane_stride_for(num_tracks);
 		op.flags = d_out_flags;
-		op.one = 1.0f;
 		const uint32_t warps = warps_for(op.plane_stride, k_object_components, context->max_dynamic_smem);
 		if (warps == 0)
 			return set_error(context, ACLB200_ERR_UNSUPPORTED, "local_to_object_space: the skeleton's object transforms do not fit in shared memory");
@@ -1160,7 +1153,6 @@ extern "C"
 			p.error_stride = uint32_t(stride / bone_stride);		// tracks a pose row holds: every job fits (checked above)
 			p.plane_stride = plane_stride;
 			p.components = components;
-			p.one = 1.0f;
 
 			build_error_requests_kernel<<<(chunk.num_poses + 255) / 256, 256, 0, cuda_stream>>>(p);
 			error = cudaGetLastError();

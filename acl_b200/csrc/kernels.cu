@@ -532,7 +532,6 @@ namespace aclb200
 			// ride along (their range is (constant, 0)) and a final select keeps the constant itself, as the reference writes it
 			// (decompression.scalar.h:289-315): no divergence between the lanes of a warp.
 			const uint32_t* pool_words = reinterpret_cast<const uint32_t*>(s_dynamic);
-			const float one = p.one;
 			const uint64_t pose_stride = p.pose_stride;
 			const uint32_t num_groups = s_num_groups;
 			for (uint32_t group = 0; group < num_groups; ++group)
@@ -639,10 +638,10 @@ namespace aclb200
 							for (int c = 0; c < COMPONENTS; ++c)
 							{
 								float2 end = mul2(make_float2(u2f(unpack(ha.y + desc.x + num_bits * c)), u2f(unpack(hb.y + desc.x + num_bits * c))), inv_max);
-								end = muladd2(end, range_extent[c], range_min[c], one);
+								end = muladd2(end, range_extent[c], range_min[c]);
 								const float2 begin = make_float2(start[c], end.x);
 								// rtm::scalar_lerp / vector_lerp: end * alpha + (start - start * alpha)
-								const float2 value = add2(mul2(end, alpha), sub2(begin, mul2(begin, alpha), one), one);
+								const float2 value = add2(mul2(end, alpha), sub2(begin, mul2(begin, alpha)));
 								store(row_a, c, constant ? range_min[c] : value.x);
 								store(row_b, c, constant ? range_min[c] : value.y);
 								start[c] = end.y;
@@ -881,7 +880,6 @@ namespace aclb200
 		// small clips: keep a block busy with at least ~4096 (request, track) items when the pool allows
 		params.requests_per_block = requests_per_block;
 		params.smem_bytes = k_scalar_pool_bytes;
-		params.one = 1.0f;
 		params.magic_tracks = division_magic(params.max_tracks == 0 ? 1 : params.max_tracks);
 	}
 

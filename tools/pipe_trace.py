@@ -1,5 +1,6 @@
 """Timeline of the pipeline kernel's hand-overs (development helper, GPU box): needs a library built with -DACLB200_PIPE_TRACE=1
-(ACLB200_LIB=build_variants/lib_trace.so python tools/pipe_trace.py [--clips N] [--math exact|fast]).
+(ACLB200_OUT=$PWD/lib_trace.so sh acl_b200/csrc/build.sh -DACLB200_PIPE_TRACE=1, then
+ACLB200_LIB=$PWD/lib_trace.so python tools/pipe_trace.py [--clips N] [--math exact|fast]).
 Stamps per (block, iteration), SM clock cycles: 0 consumer starts waiting for the stage, 1 stage full, 2 last chunk decoded,
 3 consumers' barrier passed, 4 stores handed to the TMA unit, 5 stores have read shared memory, 6 next loads issued, 7 seek done."""
 import argparse, json, os, sys
