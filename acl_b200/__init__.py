@@ -6,7 +6,7 @@ ctypes binding the tests and bench.py drive it through; it holds no decode logic
 importing it without the built library, or creating a Context without a CUDA device, raises.
 """
 from .api import (  # noqa: F401
-    AclB200Error, Context, ClipSet, Options, library_path, make_requests,
+    AclB200Error, Context, ClipSet, Database, Options, library_path, make_requests, TIER_MEDIUM, TIER_LOW,
     ROUND_NONE, ROUND_FLOOR, ROUND_CEIL, ROUND_NEAREST, ROUND_PER_TRACK,
     LOOP_CLAMP, LOOP_WRAP, LOOP_AS_COMPRESSED,
     NORMALIZE_NEVER, NORMALIZE_LERP_ONLY, NORMALIZE_ALWAYS,

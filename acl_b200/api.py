@@ -17,6 +17,7 @@ LAYOUT_QVV48, LAYOUT_QVV40 = 0, 1
 MATH_EXACT, MATH_FAST = 0, 1
 SKIP_ROTATION, SKIP_TRANSLATION, SKIP_SCALE = 1, 2, 4
 TRACK_QVVF = 12
+TIER_MEDIUM, TIER_LOW = 1, 2
 
 # numpy view of aclb200_request {uint32 clip; float sample_time}
 REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32)])
@@ -83,6 +84,11 @@ class _ClipsetInfo(C.Structure):
                 ("blob_bytes", C.c_uint64), ("index_bytes", C.c_uint64)]
 
 
+class _DatabaseInfo(C.Structure):
+    _fields_ = [("num_chunks", C.c_uint32 * 2), ("bulk_data_size", C.c_uint32 * 2), ("max_chunk_size", C.c_uint32), ("num_clips", C.c_uint32),
+                ("num_segments", C.c_uint32), ("is_bulk_data_inline", C.c_uint32), ("hash", C.c_uint32), ("size", C.c_uint32)]
+
+
 class _ClipInfo(C.Structure):
     _fields_ = [("num_tracks", C.c_uint32), ("num_samples", C.c_uint32), ("sample_rate", C.c_float), ("duration", C.c_float),
                 ("num_segments", C.c_uint32), ("looping_policy", C.c_uint32), ("hash", C.c_uint32), ("size", C.c_uint32)]
@@ -133,6 +139,14 @@ def _lib():
         l.aclb200_set_error_chunk_bytes.argtypes = [vp, u64]
         l.aclb200_decompress_all_samples.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp]
         l.aclb200_local_to_object_space.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp]
+        l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
+        l.aclb200_release_database.argtypes = [vp, vp]
+        l.aclb200_release_database.restype = None
+        l.aclb200_database_get_info.argtypes = [vp, C.POINTER(_DatabaseInfo)]
+        l.aclb200_database_get_loaded_chunks.argtypes = [vp, u32, C.POINTER(u32)]
+        l.aclb200_database_stream_in.argtypes = [vp, vp, u32, u32, vp, C.POINTER(u32), vp]
+        l.aclb200_database_stream_out.argtypes = [vp, vp, u32, u32, C.POINTER(u32), vp]
+        l.aclb200_clipset_bind_database.argtypes = [vp, vp, vp, C.POINTER(u32)]
         l.aclb200_launch_count.argtypes = [vp]
         l.aclb200_launch_count.restype = u64
         _lib_handle = l
@@ -149,7 +163,8 @@ def exported_symbols() -> list[str]:
         "aclb200_debug_seek", "aclb200_debug_unpack", "aclb200_debug_set_trace", "aclb200_launch_count",
         "aclb200_device_malloc", "aclb200_device_free", "aclb200_copy_to_device", "aclb200_copy_to_host",
         "aclb200_calculate_compression_error", "aclb200_set_error_chunk_bytes", "aclb200_local_to_object_space",
-        "aclb200_decompress_all_samples",
+        "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
+        "aclb200_database_get_loaded_chunks", "aclb200_database_stream_in", "aclb200_database_stream_out", "aclb200_clipset_bind_database",
     ]
 
 
@@ -204,9 +219,71 @@ class ClipSet:
             raise IndexError(clip)
         return info
 
+    def bind_database(self, database: "Database | None") -> None:
+        """decompression_context::initialize(tracks, database) for every clip (None unbinds). A clip the database does not contain
+        raises AclB200Error with .failed_clip set."""
+        failed = C.c_uint32(0xFFFFFFFF)
+        status = _lib().aclb200_clipset_bind_database(self._context._handle, self._handle, database._handle if database else None, C.byref(failed))
+        if status != 0:
+            error = AclB200Error(status, _lib().aclb200_last_error(self._context._handle).decode())
+            error.failed_clip = failed.value
+            raise error
+        self._database = database       # the database must outlive the binding
+
     def release(self) -> None:
         if self._handle:
             _lib().aclb200_release_clipset(self._context._handle, self._handle)
+            self._handle = 0
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
+class Database:
+    """aclb200_database: a compressed_database on the device, its tiers streamed in and out in chunks."""
+
+    def __init__(self, context: "Context", handle: int):
+        self._context = context
+        self._handle = handle
+
+    def info(self) -> _DatabaseInfo:
+        info = _DatabaseInfo()
+        _lib().aclb200_database_get_info(self._handle, C.byref(info))
+        return info
+
+    def loaded_chunks(self, tier: int) -> int:
+        loaded = C.c_uint32()
+        self._context._check(_lib().aclb200_database_get_loaded_chunks(self._handle, tier, C.byref(loaded)))
+        return loaded.value
+
+    def is_streamed_in(self, tier: int) -> bool:
+        return self.loaded_chunks(tier) == self.info().num_chunks[tier - 1]
+
+    def stream_in(self, tier: int, num_chunks: int = 0xFFFFFFFF, bulk_data: np.ndarray | None = None, stream=None) -> int:
+        """database_context::stream_in(tier, num_chunks); bulk_data = the tier's whole bulk data, None for inline bulk data.
+        Returns the number of chunks streamed in."""
+        if bulk_data is not None:
+            bulk_data = np.ascontiguousarray(bulk_data, dtype=np.uint8)
+            if bulk_data.nbytes < self.info().bulk_data_size[tier - 1]:
+                raise ValueError("bulk_data must hold the tier's whole bulk data")
+        count = C.c_uint32()
+        self._context._check(_lib().aclb200_database_stream_in(self._context._handle, self._handle, tier, num_chunks,
+                                                               None if bulk_data is None else bulk_data.ctypes.data, C.byref(count),
+                                                               _stream_ptr(stream)))
+        return count.value
+
+    def stream_out(self, tier: int, num_chunks: int = 0xFFFFFFFF, stream=None) -> int:
+        count = C.c_uint32()
+        self._context._check(_lib().aclb200_database_stream_out(self._context._handle, self._handle, tier, num_chunks, C.byref(count),
+                                                                _stream_ptr(stream)))
+        return count.value
+
+    def release(self) -> None:
+        if self._handle:
+            _lib().aclb200_release_database(self._context._handle, self._handle)
             self._handle = 0
 
     def __del__(self):
@@ -265,6 +342,12 @@ class Context:
                                                     sizes.size, int(check_hash), C.byref(handle), C.byref(failed))
         self._check(status)
         return ClipSet(self, handle.value)
+
+    def upload_database(self, blob: np.ndarray, check_hash: bool = False) -> Database:
+        """Validates and uploads a compressed_database blob (nothing streamed in yet)."""
+        handle = C.c_void_p()
+        self._check(_lib().aclb200_upload_database(self._handle, blob.ctypes.data, blob.size, int(check_hash), C.byref(handle)))
+        return Database(self, handle.value)
 
     # ---- device entry points: every pointer is a torch CUDA tensor (or a raw device address) ----
     def decompress_tracks(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, stream=None) -> None:

@@ -91,7 +91,17 @@ namespace aclb200
 			// ... and so must skipped sub-tracks (track_writer::skip_*)
 			const bool any_masked = (options->skip_mask & 7u) != 0 || options->d_skip_track_mask != nullptr;
 			const bool tracks_launch = is_transform && !single_track;
-			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked);
+			// a bound database with chunks streamed in: the launch takes the database kernels (with nothing streamed in, the resident key
+			// frames give the reference's result, so every other launch runs the kernels it always did)
+			const bool database = is_transform && database_streamed_in(clipset);
+			if (database)
+			{
+				params.db_first_segment = clipset->d_db_first_segment;
+				params.db_tiers = clipset->database->d_tiers;
+				params.db_bulk[0] = clipset->database->d_bulk[0];
+				params.db_bulk[1] = clipset->database->d_bulk[1];
+			}
+			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database);
 			return ACLB200_OK;
 		}
 
@@ -110,7 +120,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.3 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.4 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -228,6 +238,7 @@ extern "C"
 			return;
 		cudaSetDevice(clipset->device);
 		release_base_poses(clipset);
+		cudaFree(clipset->d_db_first_segment);
 		cudaFree(clipset->d_data);
 		cudaFree(clipset->d_clips);
 		delete clipset;
@@ -266,6 +277,8 @@ extern "C"
 		if (status != ACLB200_OK || num_requests == 0)
 			return status;
 		cudaSetDevice(context->device);
+		if (params.db_tiers != nullptr)
+			return finish_launch(context, launch_transform_decompress_tracks_database(params, static_cast<cudaStream_t>(stream)), "decompress_tracks (database)");
 
 		// Main path: the persistent TMA pipeline (pipeline.cu). It assembles whole poses in shared memory, so launches that must
 		// leave `skipped` default sub-tracks untouched, or whose poses do not fit in shared memory, use the plain kernels instead.
@@ -303,6 +316,8 @@ extern "C"
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null track index pointer");
 		params.track_indices = d_track_indices;
 		cudaSetDevice(context->device);
+		if (params.db_tiers != nullptr)
+			return finish_launch(context, launch_transform_decompress_track_database(params, static_cast<cudaStream_t>(stream)), "decompress_track (database)");
 		return finish_launch(context, launch_transform_decompress_track(params, options->math_mode, static_cast<cudaStream_t>(stream)), "decompress_track");
 	}
 
@@ -445,6 +460,8 @@ extern "C"
 		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, true, params);
 		if (status != ACLB200_OK || num_requests == 0)
 			return status;
+		if (params.db_tiers != nullptr)
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "debug_seek: the clip set's database has chunks streamed in");
 		cudaSetDevice(context->device);
 		return finish_launch(context, launch_transform_debug_seek(params, d_out, static_cast<cudaStream_t>(stream)), "debug_seek");
 	}
@@ -459,6 +476,8 @@ extern "C"
 			return status;
 		if (which > 1)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "key frame selector must be 0 or 1");
+		if (params.db_tiers != nullptr)
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "debug_unpack: the clip set's database has chunks streamed in");
 		params.debug_which = which;
 		params.debug_max_sub_tracks = max_animated_sub_tracks;
 		cudaSetDevice(context->device);

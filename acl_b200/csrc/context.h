@@ -76,16 +76,43 @@ struct aclb200_clipset
 	uint8_t* d_data = nullptr;
 	aclb200::ClipDesc* d_clips = nullptr;
 
+	// aclb200_clipset_bind_database (database.cpp)
+	const aclb200_database* database = nullptr;
+	uint32_t* d_db_first_segment = nullptr;			// [num_clips] first database segment of each clip, 0xFFFFFFFF when it has none
+	std::vector<uint32_t> host_blob_db_offset;		// [num_clips] clip_header_offset of its tracks_database_header, 0xFFFFFFFF without one
+	std::vector<std::vector<uint32_t>> host_db_pose_bits;	// animated_pose_bit_size of each segment of the clips bound to a database
+
 	// base pose rows built on first use per (layout, normalisation, default modes, default values), a handful kept
 	mutable std::mutex base_mutex;
 	mutable std::vector<aclb200::BasePoseRows> base_rows;
 	mutable uint64_t base_clock = 0;
 };
 
+// A compressed_database on the device (database.cpp): the blob's headers stay on the host, the tier metadata and the streamed in
+// bulk data live in HBM.
+struct aclb200_database
+{
+	int device = 0;
+	std::vector<uint8_t> blob;						// the compressed_database buffer (with its inline bulk data, if any)
+	aclb200_database_info info = {};
+	std::vector<uint32_t> clip_hash;				// per database clip, in runtime header order
+	std::vector<uint32_t> clip_header_offset;		// runtime clip header offset of each clip (database_clip_metadata::clip_header_offset)
+	std::vector<uint32_t> clip_first_segment;		// first database segment of each clip
+	std::vector<uint32_t> clip_num_segments;
+	mutable std::vector<uint32_t> segment_pose_bits;	// animated_pose_bit_size of each database segment once a clip set bound it, else 0
+	std::vector<uint64_t> host_tiers;				// [num_segments][2] host mirror of d_tiers
+	std::vector<uint32_t> loaded[2];				// loaded chunk bit sets, bit (31 - i % 32) of word i / 32 (acl::bitset)
+	std::vector<std::vector<uint32_t>> chunk_segments[2];	// per tier and chunk: the segments whose metadata the streamed in chunk published
+	unsigned long long* d_tiers = nullptr;			// [num_segments][2] database_runtime_segment_header::tier_metadata
+	uint8_t* d_bulk[2] = { nullptr, nullptr };		// tier buffers (allocated while a chunk of the tier is streamed in)
+};
+
 namespace aclb200
 {
 	aclb200_status set_error(aclb200_context* context, aclb200_status status, const std::string& message);
 	aclb200_status check_cuda(aclb200_context* context, cudaError_t error, const char* what);
+	// database.cpp: the clip set is bound to a database with at least one chunk streamed in (the launch takes the database kernels)
+	bool database_streamed_in(const aclb200_clipset* clipset);
 
 	// One launch description shared by every kernel of the transform / scalar paths.
 	struct DecodeParams
@@ -140,13 +167,19 @@ namespace aclb200
 		uint32_t layout;
 		uint32_t debug_which;
 		uint32_t debug_max_sub_tracks;
+		// the database kernels (a clip set bound to a database with chunks streamed in, database.cpp)
+		const uint32_t* db_first_segment;			// [num_clips] the clip's first database segment, 0xFFFFFFFF when it has none
+		const unsigned long long* db_tiers;			// [database segments][2] tier metadata: (samples_offset << 32) | sample_indices
+		const uint8_t* db_bulk[2];					// medium, low tier buffers
 	};
 
 	// kernels.cu
-	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging);
+	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);
 	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);
 	cudaError_t launch_transform_debug_unpack(const DecodeParams& params, uint32_t* d_out, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);

@@ -1202,6 +1202,8 @@ extern "C"
 		const uint32_t* d_output_indices, const void* d_base_poses, const aclb200_options* options, aclb200_track_error* d_out_errors,
 		float* d_out_error_matrix, void* stream)
 	{
+		if (database_streamed_in(clipset))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "calculate_compression_error: the clip set's database has chunks streamed in");
 		try
 		{
 			return calculate_compression_error_impl(context, clipset, jobs, num_jobs, d_raw_poses, d_parent_indices, d_shell_distances, d_output_indices,
@@ -1279,6 +1281,8 @@ extern "C"
 	aclb200_status aclb200_decompress_all_samples(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_error_job* jobs,
 		uint32_t num_jobs, const aclb200_options* options, void* d_out, void* stream)
 	{
+		if (database_streamed_in(clipset))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_all_samples: the clip set's database has chunks streamed in");
 		try
 		{
 			return decompress_all_samples_impl(context, clipset, jobs, num_jobs, options, d_out, stream);

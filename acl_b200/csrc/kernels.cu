@@ -41,14 +41,16 @@ namespace aclb200
 		// OUT_STAGED: poses are assembled in shared memory and written out with full-line coalesced 16 byte stores (else every
 		//             phase stores its sub-tracks straight to global memory: needed when `skipped` default sub-tracks must keep
 		//             what the caller's buffer holds, or when a pose does not fit in shared memory)
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED>
+		// DB        : the clip set's bound database has chunks streamed in: key frames may come from its tier buffers
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
-			// dynamic shared memory: ReqState[requests_per_block] | key frame windows | pose staging
+			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
+			// dynamic shared memory: RS[requests_per_block] | key frame windows | pose staging
 			extern __shared__ __align__(16) uint8_t s_dynamic[];
 			__shared__ __align__(8) uint64_t s_barrier;
-			ReqState* s_req = reinterpret_cast<ReqState*>(s_dynamic);
+			RS* s_req = reinterpret_cast<RS*>(s_dynamic);
 			uint8_t* s_stage_bytes = s_dynamic + p.smem_stage_offset;
 			const uint32_t* s_stage = reinterpret_cast<const uint32_t*>(s_stage_bytes);
 			uint8_t* s_out = s_dynamic + p.smem_out_offset;
@@ -66,8 +68,8 @@ namespace aclb200
 			// ---- phase 1: seek + stage the two key frames ----
 			if (threadIdx.x < num_requests)
 			{
-				ReqState rs;
-				seek_transform(p, first_request + threadIdx.x, rs);
+				RS rs;
+				seek_transform<DB>(p, first_request + threadIdx.x, rs);
 				rs.out = p.out + uint64_t(first_request + threadIdx.x) * p.pose_stride;
 				if (STAGED)
 				{
@@ -85,7 +87,7 @@ namespace aclb200
 						mbar_arrive_expect_tx(&s_barrier, bytes[0] + bytes[1]);
 #pragma unroll
 						for (int k = 0; k < 2; ++k)
-							bulk_copy_g2s(s_stage_bytes + size_t(rs.word_base[k]) * 4, rs.image + rs.stream_off[k] + src_byte[k], bytes[k], &s_barrier);
+							bulk_copy_g2s(s_stage_bytes + size_t(rs.word_base[k]) * 4, stream_base(rs, k) + src_byte[k], bytes[k], &s_barrier);
 					}
 					else
 						mbar_arrive(&s_barrier);
@@ -101,7 +103,7 @@ namespace aclb200
 				{
 					const uint32_t local_request = fast_div(slot, p.magic_tracks);
 					const uint32_t bone = slot - local_request * p.max_tracks;
-					const ReqState& rs = s_req[local_request];
+					const RS& rs = s_req[local_request];
 					if (bone >= rs.num_tracks)
 						continue;
 					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
@@ -121,7 +123,7 @@ namespace aclb200
 				{
 					const uint32_t local_request = fast_div(slot, p.magic_rot);
 					const uint32_t rank = slot - local_request * p.max_animated[0];
-					const ReqState& rs = s_req[local_request];
+					const RS& rs = s_req[local_request];
 					if (rs.num_tracks == 0 || rank >= rs.num_animated[0])
 						continue;
 					float rotation[4];
@@ -142,7 +144,7 @@ namespace aclb200
 				{
 					const uint32_t local_request = fast_div(slot, p.magic_vec);
 					uint32_t rank = slot - local_request * max_vectors;
-					const ReqState& rs = s_req[local_request];
+					const RS& rs = s_req[local_request];
 					uint32_t kind = 1;
 					if (rank >= p.max_animated[1])
 					{
@@ -188,15 +190,15 @@ namespace aclb200
 		}
 
 		// decompress_track_v0, decompression.transform.h:1753-2050: one thread per request, one bone each
-		template<int NORM, bool PER_TRACK>
+		template<int NORM, bool PER_TRACK, bool DB = false>
 		__global__ void __launch_bounds__(128)
 		transform_decompress_track_kernel(const DecodeParams p)
 		{
 			const uint32_t request = blockIdx.x * blockDim.x + threadIdx.x;
 			if (request >= p.num_requests)
 				return;
-			ReqState rs;
-			seek_transform(p, request, rs);
+			typename std::conditional<DB, ReqStateDB, ReqState>::type rs;
+			seek_transform<DB>(p, request, rs);
 			const uint32_t bone = p.track_indices[request];
 			if (bone >= rs.num_tracks)
 				return;		// :1766-1768: invalid track index, nothing is written
@@ -694,52 +696,60 @@ namespace aclb200
 			return divisor <= 1 ? 0u : uint32_t((uint64_t(1) << 32) / divisor) + 1u;
 		}
 
-		template<int NORM, bool PER_TRACK>
+		template<int NORM, bool PER_TRACK, bool DB = false>
 		cudaError_t launch_tracks(const DecodeParams& params, cudaStream_t stream)
 		{
 			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
 			const bool staged = params.stage_bytes != 0;
 			const bool out_staged = params.smem_pose_bytes != 0;
 			if (staged && out_staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			else if (staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, false><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, false, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			else if (out_staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			else
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, false><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, false, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			return cudaGetLastError();
 		}
 
-		template<int NORM, bool PER_TRACK>
+		template<int NORM, bool PER_TRACK, bool DB = false>
 		cudaError_t launch_track(const DecodeParams& params, cudaStream_t stream)
 		{
 			const uint32_t blocks = (params.num_requests + 127) / 128;
-			transform_decompress_track_kernel<NORM, PER_TRACK><<<blocks, 128, 0, stream>>>(params);
+			transform_decompress_track_kernel<NORM, PER_TRACK, DB><<<blocks, 128, 0, stream>>>(params);
 			return cudaGetLastError();
 		}
 
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED>
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB>
 		cudaError_t set_smem_attribute_one(int optin_limit, int& min_available)
 		{
 			// the opt-in limit covers static + dynamic shared memory
 			cudaFuncAttributes attributes;
-			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED>);
+			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB>);
 			if (error != cudaSuccess)
 				return error;
 			const int available = optin_limit - int(attributes.sharedSizeBytes);
 			if (available < min_available)
 				min_available = available;
-			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
+			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
 		}
 
 		template<int NORM, bool PER_TRACK>
 		cudaError_t set_smem_attribute(int optin_limit, int& min_available)
 		{
-			cudaError_t error = set_smem_attribute_one<NORM, PER_TRACK, true, true>(optin_limit, min_available);
-			if (error == cudaSuccess) error = set_smem_attribute_one<NORM, PER_TRACK, true, false>(optin_limit, min_available);
-			if (error == cudaSuccess) error = set_smem_attribute_one<NORM, PER_TRACK, false, true>(optin_limit, min_available);
-			if (error == cudaSuccess) error = set_smem_attribute_one<NORM, PER_TRACK, false, false>(optin_limit, min_available);
+			cudaError_t error = cudaSuccess;
+			for (int db = 0; db < 2 && error == cudaSuccess; ++db)
+			{
+				error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, false, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, true, false, false>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, false, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, false, false, false>(optin_limit, min_available);
+			}
 			return error;
 		}
 	}
@@ -763,8 +773,9 @@ namespace aclb200
 	}
 
 	// requests_per_block, the division magics and the shared memory carve-up of a launch
-	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging)
+	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database)
 	{
+		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);
 		// ~28 KB of shared memory per block keeps 8 blocks resident per SM
@@ -778,7 +789,7 @@ namespace aclb200
 		if (requests_per_block < 1) requests_per_block = 1;
 		if (requests_per_block > k_max_requests_per_block) requests_per_block = k_max_requests_per_block;
 
-		auto bytes_needed = [&](uint32_t requests) { return requests * (uint32_t(sizeof(ReqState)) + 2 * stage_bytes + pose_bytes); };
+		auto bytes_needed = [&](uint32_t requests) { return requests * (state_bytes + 2 * stage_bytes + pose_bytes); };
 		while (requests_per_block > 1 && bytes_needed(requests_per_block) > block_budget)
 			--requests_per_block;
 		// a single request that does not fit: give up output staging first, then key frame staging
@@ -790,7 +801,7 @@ namespace aclb200
 		params.requests_per_block = requests_per_block;
 		params.stage_bytes = stage_bytes;
 		params.smem_pose_bytes = pose_bytes;
-		params.smem_stage_offset = (requests_per_block * uint32_t(sizeof(ReqState)) + 15) & ~15u;
+		params.smem_stage_offset = (requests_per_block * state_bytes + 15) & ~15u;
 		params.smem_out_offset = params.smem_stage_offset + requests_per_block * 2 * stage_bytes;
 		params.smem_bytes = params.smem_out_offset + requests_per_block * pose_bytes;
 		params.magic_tracks = division_magic(max_tracks);
@@ -819,6 +830,30 @@ namespace aclb200
 		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_track<0, true>(params, stream) : launch_track<0, false>(params, stream);
 		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_track<1, true>(params, stream) : launch_track<1, false>(params, stream);
 		default: return per_track ? launch_track<2, true>(params, stream) : launch_track<2, false>(params, stream);
+		}
+	}
+
+	// The same launches with the database instances (plan_launch(..., database = true)): both math modes run the exact kernels,
+	// as the plain kernels do
+	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream)
+	{
+		const bool per_track = params.per_track_rounding != 0;
+		switch (params.normalization)
+		{
+		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_tracks<0, true, true>(params, stream) : launch_tracks<0, false, true>(params, stream);
+		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_tracks<1, true, true>(params, stream) : launch_tracks<1, false, true>(params, stream);
+		default: return per_track ? launch_tracks<2, true, true>(params, stream) : launch_tracks<2, false, true>(params, stream);
+		}
+	}
+
+	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream)
+	{
+		const bool per_track = params.per_track_rounding != 0;
+		switch (params.normalization)
+		{
+		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_track<0, true, true>(params, stream) : launch_track<0, false, true>(params, stream);
+		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_track<1, true, true>(params, stream) : launch_track<1, false, true>(params, stream);
+		default: return per_track ? launch_track<2, true, true>(params, stream) : launch_track<2, false, true>(params, stream);
 		}
 	}
 

@@ -21,7 +21,8 @@
 //
 // Semantics kept (decompress.impl.h:66-260): initialize() returns false for an invalid / unsupported buffer, for a track type,
 // version or rotation / translation / scale format the settings do not support (a clip bound to a streaming database is accepted and
-// decodes from its resident key frames, like a reference context initialised without its database); relocated() and
+// decodes from its resident key frames, like a reference context initialised without its database; initialize(tracks, database_context)
+// binds it to a database_context below, and it then decodes from the tiers streamed in); relocated() and
 // is_bound_to() compare the hash (decompression.transform.h:134-176); seek() on an unbound context and decompress_*() before a
 // seek() do nothing; transform AND scalar clips (write_float1..4 / write_vector4); every sample_rounding_policy including per_track
 // (writer.get_rounding_policy per track); all default sub-track modes; skip_all_* / skip_track_*.
@@ -50,6 +51,7 @@
 	#include <acl/core/compressed_tracks.h>
 	#include <acl/core/track_writer.h>
 	#include <acl/decompression/decompression_settings.h>
+	#include <acl/decompression/database/database.h>
 	#include <rtm/quatf.h>
 	#include <rtm/vector4f.h>
 	#include <rtm/scalarf.h>
@@ -78,6 +80,10 @@ namespace acl_b200
 	using acl::debug_scalar_decompression_settings;
 	using acl::track_writer;
 	using acl::compressed_tracks;
+	using acl::compressed_database;
+	using acl::quality_tier;
+	using acl::database_stream_request_result;
+	using acl::default_database_settings;
 #else
 	// acl::sample_rounding_policy (core/sample_rounding_policy.h:47-107)
 	enum class sample_rounding_policy : uint32_t { none = ACLB200_ROUND_NONE, floor = ACLB200_ROUND_FLOOR, ceil = ACLB200_ROUND_CEIL, nearest = ACLB200_ROUND_NEAREST, per_track = ACLB200_ROUND_PER_TRACK };
@@ -109,6 +115,20 @@ namespace acl_b200
 		uint32_t read32(size_t offset) const { uint32_t v; std::memcpy(&v, bytes() + offset, 4); return v; }
 	};
 	inline const compressed_tracks* make_compressed_tracks(const void* buffer) { return static_cast<const compressed_tracks*>(buffer); }
+
+	// acl::compressed_database (core/compressed_database.h), acl::quality_tier (core/quality_tier.h), acl::database_stream_request_result
+	// (decompression/database/database.h:48-73) and acl::default_database_settings (database_settings.h:79-84), same names and values
+	class compressed_database
+	{
+	public:
+		uint32_t get_size() const { uint32_t v; std::memcpy(&v, this, 4); return v; }
+		uint32_t get_hash() const { uint32_t v; std::memcpy(&v, reinterpret_cast<const uint8_t*>(this) + 4, 4); return v; }
+	private:
+		compressed_database() = delete;
+	};
+	enum class quality_tier { highest_importance = 0, medium_importance = ACLB200_TIER_MEDIUM, lowest_importance = ACLB200_TIER_LOW };
+	enum class database_stream_request_result { done, dispatched, streaming_in_progress, context_not_initialized, invalid_database_tier, no_free_streaming_requests };
+	struct default_database_settings {};
 
 	// acl::decompression_settings (decompression_settings.h:74-166), same member names and defaults
 	struct decompression_settings
@@ -353,6 +373,17 @@ namespace acl_b200
 			m_clipset = nullptr;
 		}
 
+		// decompression_context::initialize(tracks, database) for the clips of the batch (NULL unbinds): false, and the offending clip, when
+		// the database does not contain a clip bound to a database
+		bool bind_database(const aclb200_database* database, uint32_t* out_failed_clip = nullptr)
+		{
+			const aclb200_status status = aclb200_clipset_bind_database(m_device->get(), m_clipset, database, out_failed_clip);
+			if (status == ACLB200_ERR_INVALID_CLIP)
+				return false;
+			m_device->check(status, "aclb200_clipset_bind_database");
+			return true;
+		}
+
 		device_context& device() const { return *m_device; }
 		const aclb200_clipset_info& info() const { return m_info; }
 		const aclb200_clipset* clipset() const { return m_clipset; }
@@ -382,6 +413,105 @@ namespace acl_b200
 		device_context* m_device;
 		aclb200_clipset* m_clipset = nullptr;
 		aclb200_clipset_info m_info = {};
+	};
+
+	// Drop-in for acl::database_context<database_settings> (decompression/database/database.h:85-170) over a database whose bulk data is
+	// inline: initialize() streams every chunk in, as the reference's streamer-less initialize does (database.impl.h:91-212), and
+	// stream_in / stream_out(tier, n) then move chunks of the inline bulk data in and out of HBM (aclb200_database_stream_in / _out).
+	template<class database_settings_type = default_database_settings>
+	class database_context
+	{
+	public:
+		database_context() : m_device(&device_context::default_device()) {}
+		explicit database_context(device_context& device) : m_device(&device) {}
+		~database_context() { reset(); }
+		database_context(const database_context&) = delete;
+		database_context& operator=(const database_context&) = delete;
+
+		// false for an invalid database or one whose bulk data is not inline (the reference asserts and returns false, :95-102)
+		bool initialize(const compressed_database& database)
+		{
+			if (is_initialized())
+				return false;
+			aclb200_database* handle = nullptr;
+			const aclb200_status status = aclb200_upload_database(m_device->get(), &database, database.get_size(), 0, &handle);
+			if (status == ACLB200_ERR_INVALID_CLIP)
+				return false;
+			m_device->check(status, "aclb200_upload_database");
+			m_device->check(aclb200_database_get_info(handle, &m_info), "aclb200_database_get_info");
+			if (!m_info.is_bulk_data_inline)
+			{
+				aclb200_release_database(m_device->get(), handle);
+				return false;
+			}
+			m_database = &database;
+			m_handle = handle;
+			for (uint32_t tier = ACLB200_TIER_MEDIUM; tier <= ACLB200_TIER_LOW; ++tier)
+				if (m_info.num_chunks[tier - 1] != 0)
+					m_device->check(aclb200_database_stream_in(m_device->get(), m_handle, tier, ~0u, nullptr, nullptr, nullptr), "aclb200_database_stream_in");
+			return true;
+		}
+		void reset()
+		{
+			if (m_handle != nullptr)
+				aclb200_release_database(m_device->get(), m_handle);
+			m_handle = nullptr;
+			m_database = nullptr;
+		}
+		bool is_initialized() const { return m_handle != nullptr; }
+		const compressed_database* get_compressed_database() const { return m_database; }
+
+		// database_context::contains, database.impl.h:369-405: the clip is bound to a database and its runtime clip header holds its hash
+		bool contains(const compressed_tracks& tracks) const
+		{
+			if (!is_initialized())
+				return false;
+			const uint8_t* clip = reinterpret_cast<const uint8_t*>(&tracks);
+			const uint8_t* db = reinterpret_cast<const uint8_t*>(m_database);
+			if ((read32(clip + 28) & (1u << 8)) == 0)		// tracks_header::misc_packed bit 8, has_database
+				return false;
+			const uint32_t clip_header_offset = read32(clip + 32 + read32(clip + 32 + 32));	// transform_tracks_header::database_header_offset
+			const uint32_t clip_metadata = 8 + read32(db + 8 + 28);
+			for (uint32_t index = 0; index < m_info.num_clips; ++index)
+				if (read32(db + clip_metadata + index * 8 + 4) == clip_header_offset && read32(db + clip_metadata + index * 8) == tracks.get_hash())
+					return true;
+			return false;
+		}
+		bool is_streamed_in(quality_tier tier) const
+		{
+			uint32_t loaded = 0;
+			if (!is_initialized() || aclb200_database_get_loaded_chunks(m_handle, static_cast<uint32_t>(tier), &loaded) != ACLB200_OK)
+				return false;
+			return loaded == m_info.num_chunks[static_cast<uint32_t>(tier) - 1];
+		}
+		bool is_streaming(quality_tier) const { return false; }		// requests complete before stream_in / stream_out return
+		database_stream_request_result stream_in(quality_tier tier, uint32_t num_chunks_to_stream = ~0u) { return stream(tier, num_chunks_to_stream, true); }
+		database_stream_request_result stream_out(quality_tier tier, uint32_t num_chunks_to_stream = ~0u) { return stream(tier, num_chunks_to_stream, false); }
+
+		const aclb200_database* handle() const { return m_handle; }
+
+	private:
+		static uint32_t read32(const uint8_t* p) { uint32_t v; std::memcpy(&v, p, 4); return v; }
+		database_stream_request_result stream(quality_tier tier, uint32_t num_chunks, bool in)
+		{
+			if (!is_initialized())
+				return database_stream_request_result::context_not_initialized;
+			const uint32_t index = static_cast<uint32_t>(tier);
+			if (index != ACLB200_TIER_MEDIUM && index != ACLB200_TIER_LOW)
+				return database_stream_request_result::invalid_database_tier;
+			if (m_info.num_chunks[index - 1] == 0)
+				return database_stream_request_result::done;		// database.impl.h:485-486: nothing to stream
+			uint32_t count = 0;
+			const aclb200_status status = in ? aclb200_database_stream_in(m_device->get(), m_handle, index, num_chunks, nullptr, &count, nullptr)
+				: aclb200_database_stream_out(m_device->get(), m_handle, index, num_chunks, &count, nullptr);
+			m_device->check(status, in ? "aclb200_database_stream_in" : "aclb200_database_stream_out");
+			return count != 0 ? database_stream_request_result::dispatched : database_stream_request_result::done;
+		}
+
+		device_context* m_device;
+		const compressed_database* m_database = nullptr;
+		aclb200_database* m_handle = nullptr;
+		aclb200_database_info m_info = {};
 	};
 
 	// Where a batch writes its poses: device memory, request r at d_poses + r * pose_stride_bytes (0 = packed)
@@ -516,6 +646,20 @@ namespace acl_b200
 			const aclb200_clipset_info& info = batch().info();
 			m_components = info.track_type == ACLB200_TRACK_QVVF ? 12u : (info.track_type <= 3 ? info.track_type + 1 : 4u);
 			m_pose.assign(size_t(info.max_tracks) * m_components, 0.0F);
+			return true;
+		}
+		// initialize(tracks, database), decompress.impl.h:85-110: false when the database does not contain the clip; the clip then decodes
+		// from the tiers of `database` streamed in, at the time of each decompress call
+		template<class database_settings_type>
+		bool initialize(const compressed_tracks& tracks, const database_context<database_settings_type>& database)
+		{
+			if (!database.is_initialized() || !database.contains(tracks) || !initialize(tracks))
+				return false;
+			if (!batch().bind_database(database.handle()))
+			{
+				reset();
+				return false;
+			}
 			return true;
 		}
 		// a raw buffer holding a compressed_tracks instance

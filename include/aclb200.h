@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 3
+#define ACLB200_VERSION_MINOR 4
 
 typedef enum aclb200_status
 {
@@ -76,6 +76,7 @@ enum
 
 typedef struct aclb200_context aclb200_context;
 typedef struct aclb200_clipset aclb200_clipset;
+typedef struct aclb200_database aclb200_database;
 
 /* One decompression request == one `context.initialize(clip); context.seek(sample_time, policy);
  * context.decompress_tracks(writer);` sequence of the reference (decompress.h:90-172). */
@@ -204,6 +205,57 @@ ACLB200_API aclb200_status aclb200_clipset_get_info(const aclb200_clipset* clips
 /* compressed_tracks accessors (compressed_tracks.h:60-140) */
 ACLB200_API aclb200_status aclb200_clipset_get_clip_info(const aclb200_clipset* clipset, uint32_t clip, aclb200_clip_info* out_info);
 
+/* ---- Streaming databases: acl::compressed_database + acl::database_context (decompression/database/database.h) ----
+ * A clip built with acl::build_database keeps its most important key frames; the rest sit in a compressed_database, split into a medium
+ * and a low importance tier of fixed-size chunks. Once its clip set is bound to the database, a clip decodes from whatever key frames
+ * of the tiers are streamed in, exactly as a decompression_context initialised with a database_context does.
+ *
+ * Ordering: stream_in / stream_out enqueue their device work on `stream`. A decode enqueued on the same stream after the call sees the
+ * new tier state; one enqueued before it does not. Work on another stream must wait for an event recorded after the call, as for every
+ * other call of this library. A database must outlive the clip sets bound to it and the launches that read it. */
+
+/* acl::quality_tier (core/quality_tier.h): the tiers a database stores */
+enum { ACLB200_TIER_MEDIUM = 1, ACLB200_TIER_LOW = 2 };
+
+typedef struct aclb200_database_info
+{
+	uint32_t num_chunks[2];			/* compressed_database::get_num_chunks(medium / low) */
+	uint32_t bulk_data_size[2];		/* get_bulk_data_size(medium / low) */
+	uint32_t max_chunk_size;		/* get_max_chunk_size() */
+	uint32_t num_clips;				/* get_num_clips() */
+	uint32_t num_segments;			/* get_num_segments() */
+	uint32_t is_bulk_data_inline;	/* is_bulk_data_inline() */
+	uint32_t hash;					/* get_hash() */
+	uint32_t size;					/* get_size() */
+} aclb200_database_info;
+
+/* compressed_database::is_valid(check_hash) + the version check (core/impl/compressed_database.impl.h:142-162), plus bounds checks of
+ * every chunk description, clip metadata entry and runtime segment header offset. A corrupt database fails with
+ * ACLB200_ERR_INVALID_CLIP. The blob is copied: the caller may free it afterwards. Nothing is streamed in yet. */
+ACLB200_API aclb200_status aclb200_upload_database(aclb200_context* context, const void* blob, uint32_t size, uint32_t check_hash,
+	aclb200_database** out_database);
+/* Waits for the device, then frees the database. */
+ACLB200_API void aclb200_release_database(aclb200_context* context, aclb200_database* database);
+ACLB200_API aclb200_status aclb200_database_get_info(const aclb200_database* database, aclb200_database_info* out_info);
+/* Number of chunks of `tier` streamed in; database_context::is_streamed_in(tier) is loaded == num_chunks (database.impl.h:407-423). */
+ACLB200_API aclb200_status aclb200_database_get_loaded_chunks(const aclb200_database* database, uint32_t tier, uint32_t* out_loaded_chunks);
+/* database_context::stream_in(tier, num_chunks) (database.impl.h:443-523): picks the same chunk range (up to num_chunks chunks after
+ * the last loaded one), copies it to the device and publishes the tier metadata of every segment in those chunks. `host_bulk_data` holds
+ * the tier's whole bulk data (get_bulk_data_size(tier) bytes), or is NULL to use the bulk data inline in the database blob. Returns
+ * once the host bytes have been read; *out_num_chunks (may be NULL) receives the number of chunks streamed (0: nothing left to do).
+ * A tier with no chunks is an invalid argument. */
+ACLB200_API aclb200_status aclb200_database_stream_in(aclb200_context* context, aclb200_database* database, uint32_t tier, uint32_t num_chunks,
+	const void* host_bulk_data, uint32_t* out_num_chunks, void* stream);
+/* database_context::stream_out(tier, num_chunks) (database.impl.h:525-637): unpublishes the first loaded chunks; the tier buffer is freed,
+ * in stream order, with its last chunk. */
+ACLB200_API aclb200_status aclb200_database_stream_out(aclb200_context* context, aclb200_database* database, uint32_t tier, uint32_t num_chunks,
+	uint32_t* out_num_chunks, void* stream);
+/* decompression_context::initialize(tracks, database) (decompress.impl.h:85-110) for every clip of the set: each clip bound to a database
+ * (compressed_tracks::has_database) must be contained in `database`, else the call fails with ACLB200_ERR_INVALID_CLIP, names the first
+ * such clip in *out_failed_clip and leaves the binding as it was. Clips without a database are unaffected. NULL unbinds. */
+ACLB200_API aclb200_status aclb200_clipset_bind_database(aclb200_context* context, aclb200_clipset* clipset, const aclb200_database* database,
+	uint32_t* out_failed_clip);
+
 /* Replaces seek() + decompress_tracks(writer) (decompress.h:147-166; seek_v0 + decompress_tracks_v0,
  * decompression.transform.h:206-563,1526-1737) for `num_requests` requests in one fused kernel.
  * `d_requests` and `d_out` are device pointers; pose r starts at d_out + r * pose_stride_bytes and holds
@@ -302,7 +354,8 @@ typedef struct aclb200_error_job
  *   d_out_error_matrix device, optional: the error of every bone of every pose, row (poses of the earlier jobs + s) of
  *                     pose_stride_bytes / 48 floats (= max_tracks by default; scalar clip sets: tracks per row)
  * rtm::quat_normalize's rsqrtss estimate is CPU specific: errors agree with a given CPU's
- * within 5e-5 on poses tens of units across, not bit for bit (see error_metric.cu). Asynchronous on `stream`; uses scratch owned by the context. */
+ * within 5e-5 on poses tens of units across, not bit for bit (see error_metric.cu). Asynchronous on `stream`; uses scratch owned by the context.
+ * A clip set whose bound database has chunks streamed in is refused with ACLB200_ERR_UNSUPPORTED: these measurements never ignore tiers. */
 ACLB200_API aclb200_status aclb200_calculate_compression_error(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_error_job* jobs,
 	uint32_t num_jobs, const void* d_raw_poses, const uint32_t* d_parent_indices, const float* d_shell_distances,
 	const uint32_t* d_output_indices, const void* d_base_poses, const aclb200_options* options, aclb200_track_error* d_out_errors,
@@ -313,7 +366,8 @@ ACLB200_API aclb200_status aclb200_calculate_compression_error(aclb200_context* 
  * Job j contributes num_samples poses, sample i sought at min(i / sample_rate, duration) with options->rounding_policy (the reference
  * uses `nearest` "to land directly on a sample") and decoded like aclb200_decompress_tracks / aclb200_scalar_decompress_tracks would:
  * the poses of the jobs follow one another in d_out (pose stride and layout from `options`). Only clip, num_samples, sample_rate and
- * duration of a job are read. jobs is a HOST array; asynchronous on `stream`; uses scratch owned by the context. */
+ * duration of a job are read. jobs is a HOST array; asynchronous on `stream`; uses scratch owned by the context.
+ * ACLB200_ERR_UNSUPPORTED on a clip set whose bound database has chunks streamed in. */
 ACLB200_API aclb200_status aclb200_decompress_all_samples(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_error_job* jobs,
 	uint32_t num_jobs, const aclb200_options* options, void* d_out, void* stream);
 
@@ -331,7 +385,8 @@ ACLB200_API aclb200_status aclb200_local_to_object_space(aclb200_context* contex
  *  - aclb200_debug_seek: the state seek_v0 computes, one aclb200_seek_state per request (device output).
  *  - aclb200_debug_unpack: for request r and key frame `which` (0/1), writes one uint4 per animated sub-track
  *    (rotations, translations, scales order): x, y, z quantised integers (or raw float bits) and the stored
- *    per-track bit count, at d_out + r * max_animated_sub_tracks * 16 bytes. */
+ *    per-track bit count, at d_out + r * max_animated_sub_tracks * 16 bytes.
+ * Both return ACLB200_ERR_UNSUPPORTED on a clip set whose bound database has chunks streamed in. */
 ACLB200_API aclb200_status aclb200_debug_seek(aclb200_context* context, const aclb200_clipset* clipset,
 	const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options, aclb200_seek_state* d_out, void* stream);
 ACLB200_API aclb200_status aclb200_debug_unpack(aclb200_context* context, const aclb200_clipset* clipset,
