@@ -89,6 +89,23 @@ class _DatabaseInfo(C.Structure):
                 ("num_segments", C.c_uint32), ("is_bulk_data_inline", C.c_uint32), ("hash", C.c_uint32), ("size", C.c_uint32)]
 
 
+KERNEL_NONE, KERNEL_PLAIN, KERNEL_PIPELINE, KERNEL_DATABASE = 0, 1, 2, 3
+
+
+class LaunchInfo(C.Structure):
+    """aclb200_launch_info: the kernel and plan of a context's latest decompress_tracks."""
+    _fields_ = [("kernel", C.c_uint32), ("requests_per_block", C.c_uint32), ("grid_blocks", C.c_uint32), ("num_batches", C.c_uint32),
+                ("out_bulk", C.c_uint32), ("num_requests", C.c_uint32)]
+
+    @property
+    def kernel_name(self) -> str:
+        return {KERNEL_NONE: "none", KERNEL_PLAIN: "plain", KERNEL_PIPELINE: "pipeline", KERNEL_DATABASE: "database"}[self.kernel]
+
+    def __repr__(self) -> str:
+        return (f"LaunchInfo(kernel={self.kernel_name}, rpb={self.requests_per_block}, grid={self.grid_blocks}, "
+                f"batches={self.num_batches}, out_bulk={self.out_bulk}, requests={self.num_requests})")
+
+
 class _ClipInfo(C.Structure):
     _fields_ = [("num_tracks", C.c_uint32), ("num_samples", C.c_uint32), ("sample_rate", C.c_float), ("duration", C.c_float),
                 ("num_segments", C.c_uint32), ("looping_policy", C.c_uint32), ("hash", C.c_uint32), ("size", C.c_uint32)]
@@ -130,6 +147,7 @@ def _lib():
         l.aclb200_debug_seek.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp]
         l.aclb200_debug_unpack.argtypes = [vp, vp, vp, u32, C.POINTER(Options), u32, u32, vp, vp]
         l.aclb200_debug_set_trace.argtypes = [vp, vp, u32, u32]
+        l.aclb200_debug_last_launch.argtypes = [vp, C.POINTER(LaunchInfo)]
         l.aclb200_device_malloc.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
         l.aclb200_device_free.argtypes = [vp, vp]
         l.aclb200_device_free.restype = None
@@ -160,7 +178,7 @@ def exported_symbols() -> list[str]:
         "aclb200_last_error", "aclb200_upload_clips", "aclb200_upload_clips_packed", "aclb200_release_clipset",
         "aclb200_clipset_get_info", "aclb200_clipset_get_clip_info", "aclb200_decompress_tracks", "aclb200_decompress_track",
         "aclb200_scalar_decompress_tracks", "aclb200_scalar_decompress_track", "aclb200_decompress_tracks_host",
-        "aclb200_debug_seek", "aclb200_debug_unpack", "aclb200_debug_set_trace", "aclb200_launch_count",
+        "aclb200_debug_seek", "aclb200_debug_unpack", "aclb200_debug_set_trace", "aclb200_debug_last_launch", "aclb200_launch_count",
         "aclb200_device_malloc", "aclb200_device_free", "aclb200_copy_to_device", "aclb200_copy_to_host",
         "aclb200_calculate_compression_error", "aclb200_set_error_chunk_bytes", "aclb200_local_to_object_space",
         "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
@@ -376,6 +394,12 @@ class Context:
 
     def debug_set_trace(self, d_trace, num_blocks: int, num_iterations: int) -> None:
         self._check(_lib().aclb200_debug_set_trace(self._handle, _device_ptr(d_trace), num_blocks, num_iterations))
+
+    def debug_last_launch(self) -> LaunchInfo:
+        """Which kernel the latest decompress_tracks on this context ran, with its requests per block, grid and batch count."""
+        info = LaunchInfo()
+        self._check(_lib().aclb200_debug_last_launch(self._handle, C.byref(info)))
+        return info
 
     # ---- SURVEY 8(f1) / 8(f3): compression error measurement and the object space walk, poses stay on the device ----
     def calculate_compression_error(self, clipset: ClipSet, jobs: np.ndarray, d_raw_poses, d_parent_indices, d_shell_distances,

@@ -120,7 +120,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.4 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.5 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -277,8 +277,18 @@ extern "C"
 		if (status != ACLB200_OK || num_requests == 0)
 			return status;
 		cudaSetDevice(context->device);
+		// the plain and database kernels: one block per params.requests_per_block requests (kernels.cu, launch_tracks)
+		aclb200_launch_info& launch = context->last_launch;
+		launch = {};
+		launch.num_requests = num_requests;
+		launch.requests_per_block = params.requests_per_block;
+		launch.num_batches = (num_requests + params.requests_per_block - 1) / params.requests_per_block;
+		launch.grid_blocks = launch.num_batches;
 		if (params.db_tiers != nullptr)
+		{
+			launch.kernel = ACLB200_KERNEL_DATABASE;
 			return finish_launch(context, launch_transform_decompress_tracks_database(params, static_cast<cudaStream_t>(stream)), "decompress_tracks (database)");
+		}
 
 		// Main path: the persistent TMA pipeline (pipeline.cu). It assembles whole poses in shared memory, so launches that must
 		// leave `skipped` default sub-tracks untouched, or whose poses do not fit in shared memory, use the plain kernels instead.
@@ -295,12 +305,18 @@ extern "C"
 				pipeline_params.trace = context->d_trace;
 				pipeline_params.trace_blocks = context->trace_blocks;
 				pipeline_params.trace_iterations = context->trace_iterations;
+				launch.kernel = ACLB200_KERNEL_PIPELINE;
+				launch.requests_per_block = pipeline_params.requests_per_block;
+				launch.num_batches = (num_requests + pipeline_params.requests_per_block - 1) / pipeline_params.requests_per_block;
+				launch.grid_blocks = pipeline_params.grid_blocks;
+				launch.out_bulk = pipeline_params.out_bulk;
 				acquire_base_poses(clipset, pipeline_params, static_cast<cudaStream_t>(stream));
 				const cudaError_t launched = launch_transform_pipeline(pipeline_params, options->math_mode, static_cast<cudaStream_t>(stream));
 				release_base_poses_use(clipset, pipeline_params, static_cast<cudaStream_t>(stream));
 				return finish_launch(context, launched, "decompress_tracks (pipeline)");
 			}
 		}
+		launch.kernel = ACLB200_KERNEL_PLAIN;
 		return finish_launch(context, launch_transform_decompress_tracks(params, options->math_mode, static_cast<cudaStream_t>(stream)), "decompress_tracks");
 	}
 
@@ -491,6 +507,14 @@ extern "C"
 		context->d_trace = static_cast<unsigned long long*>(d_trace);
 		context->trace_blocks = d_trace != nullptr ? num_blocks : 0;
 		context->trace_iterations = d_trace != nullptr ? num_iterations : 0;
+		return ACLB200_OK;
+	}
+
+	aclb200_status aclb200_debug_last_launch(const aclb200_context* context, aclb200_launch_info* out_info)
+	{
+		if (context == nullptr || out_info == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		*out_info = context->last_launch;
 		return ACLB200_OK;
 	}
 

@@ -37,6 +37,9 @@ struct aclb200_context
 	unsigned long long* d_trace = nullptr;
 	uint32_t trace_blocks = 0;
 	uint32_t trace_iterations = 0;
+
+	// aclb200_debug_last_launch: the plan of the latest aclb200_decompress_tracks
+	aclb200_launch_info last_launch = {};
 };
 
 namespace aclb200

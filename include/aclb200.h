@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 4
+#define ACLB200_VERSION_MINOR 5
 
 typedef enum aclb200_status
 {
@@ -397,6 +397,23 @@ ACLB200_API aclb200_status aclb200_debug_unpack(aclb200_context* context, const 
  * `num_blocks` blocks record 8 clock64() stamps per batch they decode, for their first `num_iterations` batches, at
  * d_trace[(block * num_iterations + iteration) * 8 + k] (uint64). NULL switches it off. tools/pipe_trace.py reads it. */
 ACLB200_API aclb200_status aclb200_debug_set_trace(aclb200_context* context, void* d_trace, uint32_t num_blocks, uint32_t num_iterations);
+
+/* Which kernel the latest aclb200_decompress_tracks on a context launched, and the plan of that launch. Tests use it to check that
+ * a request list really reaches the pipeline configuration it was written for (several batches per block, one request per batch,
+ * the plain kernels when a pose does not fit in shared memory). */
+enum { ACLB200_KERNEL_NONE = 0, ACLB200_KERNEL_PLAIN = 1, ACLB200_KERNEL_PIPELINE = 2, ACLB200_KERNEL_DATABASE = 3 };
+
+typedef struct aclb200_launch_info
+{
+	uint32_t kernel;				/* ACLB200_KERNEL_*: NONE before the first launch with at least one request */
+	uint32_t requests_per_block;	/* requests per batch (pipeline) or per block (plain and database kernels) */
+	uint32_t grid_blocks;			/* blocks launched: the pipeline's persistent grid walks num_batches / grid_blocks batches per block */
+	uint32_t num_batches;			/* ceil(num_requests / requests_per_block) */
+	uint32_t out_bulk;				/* pipeline: 1 when pose rows leave shared memory as TMA bulk stores, 0 for 8 byte stores; 0 otherwise */
+	uint32_t num_requests;
+} aclb200_launch_info;
+
+ACLB200_API aclb200_status aclb200_debug_last_launch(const aclb200_context* context, aclb200_launch_info* out_info);
 
 /* Plain device memory helpers so that a host language without the CUDA runtime can hand device arrays (requests, variable
  * defaults, per track policies, skip masks, outputs) to the entry points above. Synchronous. */
