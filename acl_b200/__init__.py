@@ -14,4 +14,5 @@ from .api import (  # noqa: F401
     LAYOUT_QVV48, LAYOUT_QVV40, MATH_EXACT, MATH_FAST, TRACK_QVVF,
     SKIP_ROTATION, SKIP_TRANSLATION, SKIP_SCALE,
     ERROR_JOB_DTYPE, TRACK_ERROR_DTYPE, ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON,
+    OBJECT_QVVF, OBJECT_MATRIX3X4F,
 )

@@ -37,6 +37,7 @@ METRIC_QVVF, METRIC_QVVF_MATRIX3X4F = 0, 1
 ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1 = 0, 1, 2, 3
 TRACK_ERROR_DTYPE = np.dtype([("index", np.uint32), ("error", np.float32), ("sample_time", np.float32), ("flags", np.uint32)])
 ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON = 1, 2
+OBJECT_QVVF, OBJECT_MATRIX3X4F = 0, 1
 
 
 class AclB200Error(RuntimeError):
@@ -157,6 +158,7 @@ def _lib():
         l.aclb200_set_error_chunk_bytes.argtypes = [vp, u64]
         l.aclb200_decompress_all_samples.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp]
         l.aclb200_local_to_object_space.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp]
+        l.aclb200_decompress_tracks_object_space.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, u32, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -183,6 +185,7 @@ def exported_symbols() -> list[str]:
         "aclb200_calculate_compression_error", "aclb200_set_error_chunk_bytes", "aclb200_local_to_object_space",
         "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
         "aclb200_database_get_loaded_chunks", "aclb200_database_stream_in", "aclb200_database_stream_out", "aclb200_clipset_bind_database",
+        "aclb200_decompress_tracks_object_space",
     ]
 
 
@@ -371,6 +374,15 @@ class Context:
     def decompress_tracks(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, stream=None) -> None:
         self._check(_lib().aclb200_decompress_tracks(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
                                                      C.byref(options), _device_ptr(d_out), _stream_ptr(stream)))
+
+    def decompress_tracks_object_space(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices, kind: int,
+                                       d_out, d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks followed by the hierarchy walk in one kernel: 48 byte object space bones, rtm::qvvf rows (OBJECT_QVVF) or the
+        xyz lanes of a 3x4 matrix's four axes (OBJECT_MATRIX3X4F). Clip c uses the skeleton at d_parent_indices + d_skeleton_offsets[c]
+        (None: every clip at offset 0); d_out_flags (optional, uint32) receives the ERROR_FLAG_* met on the way."""
+        self._check(_lib().aclb200_decompress_tracks_object_space(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                  C.byref(options), _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                                  kind, _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     def decompress_track(self, clipset: ClipSet, d_requests, d_track_indices, num_requests: int, options: Options, d_out, stream=None) -> None:
         self._check(_lib().aclb200_decompress_track(self._handle, clipset._handle, _device_ptr(d_requests), _device_ptr(d_track_indices),

@@ -18,7 +18,8 @@ namespace aclb200
 		}
 
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
-			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params)
+			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
+			bool object_space = false)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -101,7 +102,12 @@ namespace aclb200
 				params.db_bulk[0] = clipset->database->d_bulk[0];
 				params.db_bulk[1] = clipset->database->d_bulk[1];
 			}
-			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database);
+			if (object_space && (any_skipped || any_masked))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: an object transform needs every sub-track of its parents (no skip masks, no `skipped` default mode)");
+			if (object_space && options->output_layout != ACLB200_LAYOUT_QVV48)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: the output layout must be QVV48");
+			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database,
+				object_space);
 			return ACLB200_OK;
 		}
 
@@ -120,7 +126,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.5 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.6 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -318,6 +324,40 @@ extern "C"
 		}
 		launch.kernel = ACLB200_KERNEL_PLAIN;
 		return finish_launch(context, launch_transform_decompress_tracks(params, options->math_mode, static_cast<cudaStream_t>(stream)), "decompress_tracks");
+	}
+
+	aclb200_status aclb200_decompress_tracks_object_space(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		DecodeParams params;
+		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, true);
+		if (status != ACLB200_OK)
+			return status;
+		if (object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: unknown object_kind");
+		if (d_parent_indices == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: null parent index pointer");
+		// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
+		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_object_space: one pose does not fit in a block's shared memory");
+		if (num_requests == 0)
+			return ACLB200_OK;
+		params.parent_indices = d_parent_indices;
+		params.skeleton_offsets = d_skeleton_offsets;
+		params.object_flags = d_out_flags;
+		params.object_kind = object_kind;
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		if (d_out_flags != nullptr)
+		{
+			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
+			if (cleared != cudaSuccess)
+				return check_cuda(context, cleared, "decompress_tracks_object_space");
+		}
+		return finish_launch(context, launch_transform_decompress_tracks_object_space(params, params.db_tiers != nullptr, cuda_stream),
+			"decompress_tracks_object_space");
 	}
 
 	aclb200_status aclb200_decompress_track(aclb200_context* context, const aclb200_clipset* clipset,

@@ -174,15 +174,22 @@ namespace aclb200
 		const uint32_t* db_first_segment;			// [num_clips] the clip's first database segment, 0xFFFFFFFF when it has none
 		const unsigned long long* db_tiers;			// [database segments][2] tier metadata: (samples_offset << 32) | sample_indices
 		const uint8_t* db_bulk[2];					// medium, low tier buffers
+		// the object space decode (aclb200_decompress_tracks_object_space)
+		const uint32_t* parent_indices;				// skeletons, 0xFFFFFFFF = root
+		const uint32_t* skeleton_offsets;			// [num_clips] first parent index of each clip's skeleton, or nullptr (every clip at 0)
+		uint32_t* object_flags;						// ACLB200_ERROR_FLAG_* are OR-ed in, or nullptr
+		uint32_t object_kind;						// ACLB200_OBJECT_*
 	};
 
 	// kernels.cu
-	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false);
+	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false,
+		bool force_output_staging = false);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);
 	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_tracks_object_space(const DecodeParams& params, bool database, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);
 	cudaError_t launch_transform_debug_unpack(const DecodeParams& params, uint32_t* d_out, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);

@@ -25,6 +25,7 @@
 // (the reference never fuses either: external/rtm/includes/rtm/impl/macros.vector4.impl.h:67,93,122). The results
 // are bit-identical to the reference's SSE2/AVX/scalar builds for decompress_tracks.
 #include "device_common.cuh"
+#include "object_space.cuh"
 
 #include <type_traits>
 
@@ -42,7 +43,8 @@ namespace aclb200
 		//             phase stores its sub-tracks straight to global memory: needed when `skipped` default sub-tracks must keep
 		//             what the caller's buffer holds, or when a pose does not fit in shared memory)
 		// DB        : the clip set's bound database has chunks streamed in: key frames may come from its tier buffers
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false>
+		// OBJECT    : the staged poses are taken to object space before they leave (aclb200_decompress_tracks_object_space; OUT_STAGED, QVV48)
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false, bool OBJECT = false>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
@@ -160,6 +162,26 @@ namespace aclb200
 					uint8_t* pose = OUT_STAGED ? s_out + size_t(local_request) * p.smem_pose_bytes : rs.out;
 					write_vector(p.layout, pose + size_t(bone) * p.bone_stride, kind, value);
 				}
+			}
+
+			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows ----
+			if constexpr (OBJECT)
+			{
+				static_assert(OUT_STAGED, "the object space walk runs on poses assembled in shared memory");
+				__syncthreads();
+				uint32_t flags = 0;
+				for (uint32_t local_request = threadIdx.x >> 5; local_request < num_requests; local_request += k_threads_per_block / 32)
+				{
+					const RS& rs = s_req[local_request];
+					if (rs.num_tracks == 0)
+						continue;
+					const uint32_t* parents = p.parent_indices + (p.skeleton_offsets != nullptr ? __ldg(p.skeleton_offsets + rs.clip) : 0u);
+					flags |= obj::pose_rows_to_object_space(s_out + size_t(local_request) * p.smem_pose_bytes, rs.num_tracks, parents,
+						p.object_kind == ACLB200_OBJECT_MATRIX3X4F);
+				}
+				flags = __reduce_or_sync(0xFFFFFFFFu, flags);
+				if ((threadIdx.x & 31u) == 0 && flags != 0 && p.object_flags != nullptr)
+					atomicOr(p.object_flags, flags);
 			}
 
 			// ---- phase 5: the assembled poses leave shared memory as full, coalesced 16 byte (or 8 byte) stores ----
@@ -713,6 +735,18 @@ namespace aclb200
 			return cudaGetLastError();
 		}
 
+		// The object space decode: poses are always staged in shared memory, key frames whenever they fit beside them (plan_launch)
+		template<int NORM, bool PER_TRACK, bool DB>
+		cudaError_t launch_tracks_object_space(const DecodeParams& params, cudaStream_t stream)
+		{
+			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
+			if (params.stage_bytes != 0)
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+			else
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+			return cudaGetLastError();
+		}
+
 		template<int NORM, bool PER_TRACK, bool DB = false>
 		cudaError_t launch_track(const DecodeParams& params, cudaStream_t stream)
 		{
@@ -721,18 +755,18 @@ namespace aclb200
 			return cudaGetLastError();
 		}
 
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB>
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, bool OBJECT = false>
 		cudaError_t set_smem_attribute_one(int optin_limit, int& min_available)
 		{
 			// the opt-in limit covers static + dynamic shared memory
 			cudaFuncAttributes attributes;
-			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB>);
+			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT>);
 			if (error != cudaSuccess)
 				return error;
 			const int available = optin_limit - int(attributes.sharedSizeBytes);
 			if (available < min_available)
 				min_available = available;
-			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
+			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
 		}
 
 		template<int NORM, bool PER_TRACK>
@@ -749,6 +783,10 @@ namespace aclb200
 					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false>(optin_limit, min_available);
 				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, false, true>(optin_limit, min_available)
 					: set_smem_attribute_one<NORM, PER_TRACK, false, false, false>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, true>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, true>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, true>(optin_limit, min_available);
 			}
 			return error;
 		}
@@ -773,7 +811,10 @@ namespace aclb200
 	}
 
 	// requests_per_block, the division magics and the shared memory carve-up of a launch
-	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database)
+	// force_output_staging: the object space decode needs every pose in shared memory, so a pose that does not fit gives up key frame
+	// staging instead (params.smem_bytes then tells the caller whether one request fits at all)
+	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
+		bool force_output_staging)
 	{
 		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
@@ -783,7 +824,7 @@ namespace aclb200
 
 		// bytes per staged key frame: alignment skew + the key frame + the extra word the funnel shift reads, 16 byte granular
 		uint32_t stage_bytes = max_key_frame_bytes != 0 ? ((max_key_frame_bytes + 48 + 15) & ~15u) : 0u;
-		uint32_t pose_bytes = allow_output_staging ? ((max_tracks * params.bone_stride + 15) & ~15u) : 0u;
+		uint32_t pose_bytes = allow_output_staging || force_output_staging ? ((max_tracks * params.bone_stride + 15) & ~15u) : 0u;
 
 		uint32_t requests_per_block = k_target_items_per_block / max_tracks;
 		if (requests_per_block < 1) requests_per_block = 1;
@@ -793,7 +834,7 @@ namespace aclb200
 		while (requests_per_block > 1 && bytes_needed(requests_per_block) > block_budget)
 			--requests_per_block;
 		// a single request that does not fit: give up output staging first, then key frame staging
-		if (bytes_needed(requests_per_block) > budget)
+		if (bytes_needed(requests_per_block) > budget && !force_output_staging)
 			pose_bytes = 0;
 		if (bytes_needed(requests_per_block) > budget)
 			stage_bytes = 0;
@@ -854,6 +895,24 @@ namespace aclb200
 		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_track<0, true, true>(params, stream) : launch_track<0, false, true>(params, stream);
 		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_track<1, true, true>(params, stream) : launch_track<1, false, true>(params, stream);
 		default: return per_track ? launch_track<2, true, true>(params, stream) : launch_track<2, false, true>(params, stream);
+		}
+	}
+
+	// The object space decode: both math modes run the exact kernels (the walk is IEEE exact whatever the decode does)
+	cudaError_t launch_transform_decompress_tracks_object_space(const DecodeParams& params, bool database, cudaStream_t stream)
+	{
+		const bool per_track = params.per_track_rounding != 0;
+		switch (params.normalization)
+		{
+		case ACLB200_NORMALIZE_NEVER:
+			return database ? (per_track ? launch_tracks_object_space<0, true, true>(params, stream) : launch_tracks_object_space<0, false, true>(params, stream))
+				: (per_track ? launch_tracks_object_space<0, true, false>(params, stream) : launch_tracks_object_space<0, false, false>(params, stream));
+		case ACLB200_NORMALIZE_LERP_ONLY:
+			return database ? (per_track ? launch_tracks_object_space<1, true, true>(params, stream) : launch_tracks_object_space<1, false, true>(params, stream))
+				: (per_track ? launch_tracks_object_space<1, true, false>(params, stream) : launch_tracks_object_space<1, false, false>(params, stream));
+		default:
+			return database ? (per_track ? launch_tracks_object_space<2, true, true>(params, stream) : launch_tracks_object_space<2, false, true>(params, stream))
+				: (per_track ? launch_tracks_object_space<2, true, false>(params, stream) : launch_tracks_object_space<2, false, false>(params, stream));
 		}
 	}
 

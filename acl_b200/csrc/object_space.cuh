@@ -1,0 +1,495 @@
+// acl_b200/csrc/object_space.cuh -- the hierarchy walk shared by the error measurement (error_metric.cu: object_space_kernel) and the
+// object space decode (kernels.cu: transform_decompress_tracks_kernel<..., OBJECT = true>): the reference's qvv and 3x4 matrix operations
+// restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose.
+//
+// The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
+// earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
+// wavefronts per chunk). A bone's local transform sits in the slot its object transform will take.
+#pragma once
+
+#include "context.h"
+
+#include <type_traits>
+
+namespace aclb200
+{
+	namespace obj
+	{
+		namespace
+		{
+			constexpr uint32_t k_invalid_track = 0xFFFFFFFFu;			// acl::k_invalid_track_index, core/track_types.h
+			constexpr uint32_t k_object_components = 10;				// rotation xyzw, translation xyz, scale xyz
+
+			// ---- the reference's float operations, spelled out so nothing can be contracted -------------------------------------------
+			// The measurement runs the SAME operation sequence on the raw and on the lossy pose: the two travel as one f32x2 pair
+			// (x = raw, y = lossy). Each operation is one scalar __fmul_rn / __fadd_rn / __fsub_rn per lane, intrinsics that are never
+			// contracted into an FMA. Signs: the reference xors sign masks into products and adds them; -(p) + q == q - p, p + -(q) == p - q
+			// and -(p) + -(q) == -(p + q) hold exactly in IEEE arithmetic, so the sums below are written with subtractions and no negation.
+			template<class V> struct Fp;
+
+			template<> struct Fp<float>
+			{
+				__device__ __forceinline__ float mul(float a, float b) const { return __fmul_rn(a, b); }
+				__device__ __forceinline__ float add(float a, float b) const { return __fadd_rn(a, b); }
+				__device__ __forceinline__ float sub(float a, float b) const { return __fsub_rn(a, b); }
+				__device__ __forceinline__ float splat(float a) const { return a; }
+				__device__ __forceinline__ float inv_sqrt(float a) const { return __fdiv_rn(1.0f, __fsqrt_rn(a)); }
+				__device__ __forceinline__ bool any_negative(float a, float b) const { return fminf(a, b) < 0.0f; }
+			};
+
+			template<> struct Fp<float2>
+			{
+				__device__ __forceinline__ float2 mul(float2 a, float2 b) const { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+				__device__ __forceinline__ float2 add(float2 a, float2 b) const { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+				__device__ __forceinline__ float2 sub(float2 a, float2 b) const { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+				__device__ __forceinline__ float2 splat(float a) const { return make_float2(a, a); }
+				__device__ __forceinline__ float2 inv_sqrt(float2 a) const { return make_float2(__fdiv_rn(1.0f, __fsqrt_rn(a.x)), __fdiv_rn(1.0f, __fsqrt_rn(a.y))); }
+				__device__ __forceinline__ bool any_negative(float2 a, float2 b) const { return fminf(a.x, b.x) < 0.0f || fminf(a.y, b.y) < 0.0f; }
+			};
+
+			template<class V> struct Quat { V x, y, z, w; };
+			template<class V> struct Vec3 { V x, y, z; };
+			template<class V> struct Qvv { Quat<V> rotation; Vec3<V> translation; Vec3<V> scale; };
+
+			// rtm::quat_mul, external/rtm/includes/rtm/quatf.h:498-545 (SSE2 path): (rw*l + s0*(rx*l_wzyx)) + (s1*(ry*l_zwxy) + s2*(rz*l_yxwz))
+			template<class V>
+			__device__ __forceinline__ Quat<V> quat_mul(const Fp<V>& fp, const Quat<V>& l, const Quat<V>& r)
+			{
+				Quat<V> out;
+				out.x = fp.add(fp.add(fp.mul(r.w, l.x), fp.mul(r.x, l.w)), fp.sub(fp.mul(r.y, l.z), fp.mul(r.z, l.y)));
+				out.y = fp.add(fp.sub(fp.mul(r.w, l.y), fp.mul(r.x, l.z)), fp.add(fp.mul(r.y, l.w), fp.mul(r.z, l.x)));
+				out.z = fp.add(fp.add(fp.mul(r.w, l.z), fp.mul(r.x, l.y)), fp.sub(fp.mul(r.z, l.w), fp.mul(r.y, l.x)));
+				out.w = fp.sub(fp.sub(fp.mul(r.w, l.w), fp.mul(r.x, l.x)), fp.add(fp.mul(r.y, l.y), fp.mul(r.z, l.z)));
+				return out;
+			}
+
+			// rtm::quat_mul_vector3, quatf.h:616-668 (SSE2 path): temp = conjugate(r) * (v, 0) without its W terms, result = temp * r
+			template<class V>
+			__device__ __forceinline__ Vec3<V> quat_mul_vector3(const Fp<V>& fp, const Vec3<V>& v, const Quat<V>& r)
+			{
+				const V t0 = fp.add(fp.sub(fp.mul(v.x, r.w), fp.mul(v.y, r.z)), fp.mul(v.z, r.y));
+				const V t1 = fp.sub(fp.add(fp.mul(v.x, r.z), fp.mul(v.y, r.w)), fp.mul(v.z, r.x));
+				const V t2 = fp.add(fp.sub(fp.mul(v.y, r.x), fp.mul(v.x, r.y)), fp.mul(v.z, r.w));
+				const V t3 = fp.add(fp.add(fp.mul(v.x, r.x), fp.mul(v.y, r.y)), fp.mul(v.z, r.z));
+				Vec3<V> out;
+				out.x = fp.add(fp.add(fp.mul(r.w, t0), fp.mul(r.x, t3)), fp.sub(fp.mul(r.y, t2), fp.mul(r.z, t1)));
+				out.y = fp.add(fp.sub(fp.mul(r.w, t1), fp.mul(r.x, t2)), fp.add(fp.mul(r.y, t3), fp.mul(r.z, t0)));
+				out.z = fp.add(fp.add(fp.mul(r.w, t2), fp.mul(r.x, t1)), fp.sub(fp.mul(r.z, t3), fp.mul(r.y, t0)));
+				return out;
+			}
+
+			// rtm::quat_normalize, quatf.h:917-953: dot = (x2 + z2) + (y2 + w2); IEEE 1 / sqrt in place of the rsqrtss + 2 Newton-Raphson steps
+			template<class V>
+			__device__ __forceinline__ Quat<V> quat_normalize(const Fp<V>& fp, const Quat<V>& q)
+			{
+				const V dot = fp.add(fp.add(fp.mul(q.x, q.x), fp.mul(q.z, q.z)), fp.add(fp.mul(q.y, q.y), fp.mul(q.w, q.w)));
+				const V inv_len = fp.inv_sqrt(dot);
+				Quat<V> out;
+				out.x = fp.mul(q.x, inv_len);
+				out.y = fp.mul(q.y, inv_len);
+				out.z = fp.mul(q.z, inv_len);
+				out.w = fp.mul(q.w, inv_len);
+				return out;
+			}
+
+			// ---- the negative scale branch of rtm::qvv_mul (qvvf.h:320-345): through matrices. Rare (mirrored bones), data dependent branches
+			// (quat_from_matrix), so it runs per stream on plain floats, out of line: matrix_from_qvv (matrix3x4f.h:134-159), matrix_mul (:298-321,
+			// vector_mul_add = (v0 * v1) + v2 on SSE2), matrix_remove_scale (:636-644 = vector_normalize3(axis, axis, 1e-8), vector4f.h:2310-2318),
+			// the result scale's sign bits xor-ed onto the axes, quat_from_matrix (impl/matrix_affine_common.h:153-227, its closing
+			// quat_normalize with the IEEE 1 / sqrt like every normalisation here) ----
+			struct Matrix3x4 { float m[4][3]; };
+
+			__device__ __forceinline__ Matrix3x4 matrix_from_qvv(const Qvv<float>& q)
+			{
+				const Fp<float> fp{};
+				const float x2 = fp.add(q.rotation.x, q.rotation.x), y2 = fp.add(q.rotation.y, q.rotation.y), z2 = fp.add(q.rotation.z, q.rotation.z);
+				const float xx = fp.mul(q.rotation.x, x2), xy = fp.mul(q.rotation.x, y2), xz = fp.mul(q.rotation.x, z2);
+				const float yy = fp.mul(q.rotation.y, y2), yz = fp.mul(q.rotation.y, z2), zz = fp.mul(q.rotation.z, z2);
+				const float wx = fp.mul(q.rotation.w, x2), wy = fp.mul(q.rotation.w, y2), wz = fp.mul(q.rotation.w, z2);
+				Matrix3x4 out;
+				out.m[0][0] = fp.mul(fp.sub(1.0f, fp.add(yy, zz)), q.scale.x);	out.m[0][1] = fp.mul(fp.add(xy, wz), q.scale.x);				out.m[0][2] = fp.mul(fp.sub(xz, wy), q.scale.x);
+				out.m[1][0] = fp.mul(fp.sub(xy, wz), q.scale.y);				out.m[1][1] = fp.mul(fp.sub(1.0f, fp.add(xx, zz)), q.scale.y);	out.m[1][2] = fp.mul(fp.add(yz, wx), q.scale.y);
+				out.m[2][0] = fp.mul(fp.add(xz, wy), q.scale.z);				out.m[2][1] = fp.mul(fp.sub(yz, wx), q.scale.z);				out.m[2][2] = fp.mul(fp.sub(1.0f, fp.add(xx, yy)), q.scale.z);
+				out.m[3][0] = q.translation.x;									out.m[3][1] = q.translation.y;									out.m[3][2] = q.translation.z;
+				return out;
+			}
+
+			__device__ __noinline__ void qvv_mul_negative_scale(const Qvv<float>* lhs_in, const Qvv<float>* rhs_in, Qvv<float>* out)
+			{
+				const Fp<float> fp{};
+				const Qvv<float> lhs = *lhs_in, rhs = *rhs_in;
+				const Matrix3x4 l = matrix_from_qvv(lhs), r = matrix_from_qvv(rhs);
+				float m[4][3];
+				#pragma unroll
+				for (int row = 0; row < 4; ++row)
+					#pragma unroll
+					for (int c = 0; c < 3; ++c)
+					{
+						float tmp = fp.mul(l.m[row][0], r.m[0][c]);
+						tmp = fp.add(fp.mul(l.m[row][1], r.m[1][c]), tmp);
+						tmp = fp.add(fp.mul(l.m[row][2], r.m[2][c]), tmp);
+						m[row][c] = row == 3 ? fp.add(r.m[3][c], tmp) : tmp;
+					}
+				const float scale[3] = { fp.mul(lhs.scale.x, rhs.scale.x), fp.mul(lhs.scale.y, rhs.scale.y), fp.mul(lhs.scale.z, rhs.scale.z) };
+				#pragma unroll
+				for (int axis = 0; axis < 3; ++axis)
+				{
+					const float len_sq = fp.add(fp.add(fp.mul(m[axis][0], m[axis][0]), fp.mul(m[axis][1], m[axis][1])), fp.mul(m[axis][2], m[axis][2]));
+					const float inv_len = len_sq >= 1.0e-8f ? fp.inv_sqrt(len_sq) : 1.0f;
+					const uint32_t sign = __float_as_uint(scale[axis]) & 0x80000000u;
+					#pragma unroll
+					for (int c = 0; c < 3; ++c)
+					{
+						const float normalized = len_sq >= 1.0e-8f ? fp.mul(m[axis][c], inv_len) : m[axis][c];
+						m[axis][c] = __uint_as_float(__float_as_uint(normalized) ^ sign);
+					}
+				}
+
+				Quat<float> q;
+				bool zero_axis = false;
+				#pragma unroll
+				for (int axis = 0; axis < 3; ++axis)
+					zero_axis = zero_axis || (fabsf(m[axis][0]) <= 0.00001f && fabsf(m[axis][1]) <= 0.00001f && fabsf(m[axis][2]) <= 0.00001f);
+				const float trace = fp.add(fp.add(m[0][0], m[1][1]), m[2][2]);
+				if (zero_axis)
+					q = Quat<float>{ 0.0f, 0.0f, 0.0f, 1.0f };		// Zero scale not supported, return the identity
+				else if (trace > 0.0f)
+				{
+					const float inv_trace = fp.inv_sqrt(fp.add(trace, 1.0f));
+					const float half_inv_trace = fp.mul(inv_trace, 0.5f);
+					q.x = fp.mul(fp.sub(m[1][2], m[2][1]), half_inv_trace);
+					q.y = fp.mul(fp.sub(m[2][0], m[0][2]), half_inv_trace);
+					q.z = fp.mul(fp.sub(m[0][1], m[1][0]), half_inv_trace);
+					q.w = fp.mul(__fdiv_rn(1.0f, inv_trace), 0.5f);
+					q = quat_normalize(fp, q);
+				}
+				else
+				{
+					// best axis = the largest diagonal element; the three cases are the reference's index arithmetic written out
+					const int best = m[2][2] > (m[1][1] > m[0][0] ? m[1][1] : m[0][0]) ? 2 : (m[1][1] > m[0][0] ? 1 : 0);
+					float d_best, d_next, d_next_next, s_next, s_next_next, s_w;
+					if (best == 0)		{ d_best = m[0][0]; d_next = m[1][1]; d_next_next = m[2][2]; s_next = fp.add(m[0][1], m[1][0]); s_next_next = fp.add(m[0][2], m[2][0]); s_w = fp.sub(m[1][2], m[2][1]); }
+					else if (best == 1)	{ d_best = m[1][1]; d_next = m[2][2]; d_next_next = m[0][0]; s_next = fp.add(m[1][2], m[2][1]); s_next_next = fp.add(m[1][0], m[0][1]); s_w = fp.sub(m[2][0], m[0][2]); }
+					else				{ d_best = m[2][2]; d_next = m[0][0]; d_next_next = m[1][1]; s_next = fp.add(m[2][0], m[0][2]); s_next_next = fp.add(m[2][1], m[1][2]); s_w = fp.sub(m[0][1], m[1][0]); }
+					const float pseudo_trace = fp.sub(fp.sub(fp.add(1.0f, d_best), d_next), d_next_next);
+					const float inv_pseudo_trace = fp.inv_sqrt(pseudo_trace);
+					const float half_inv_pseudo_trace = fp.mul(inv_pseudo_trace, 0.5f);
+					const float v_best = fp.mul(__fdiv_rn(1.0f, inv_pseudo_trace), 0.5f);
+					const float v_next = fp.mul(half_inv_pseudo_trace, s_next);
+					const float v_next_next = fp.mul(half_inv_pseudo_trace, s_next_next);
+					q.w = fp.mul(half_inv_pseudo_trace, s_w);
+					if (best == 0)		{ q.x = v_best; q.y = v_next; q.z = v_next_next; }
+					else if (best == 1)	{ q.y = v_best; q.z = v_next; q.x = v_next_next; }
+					else				{ q.z = v_best; q.x = v_next; q.y = v_next_next; }
+					q = quat_normalize(fp, q);
+				}
+				Qvv<float> result;
+				result.rotation = q;
+				result.translation = Vec3<float>{ m[3][0], m[3][1], m[3][2] };
+				result.scale = Vec3<float>{ scale[0], scale[1], scale[2] };
+				*out = result;
+			}
+
+			// rtm::qvv_mul(lhs, rhs), external/rtm/includes/rtm/qvvf.h:315-355, the positive scale branch (:347-353)
+			template<class V>
+			__device__ __forceinline__ Qvv<V> qvv_mul_positive(const Fp<V>& fp, const Qvv<V>& lhs, const Qvv<V>& rhs)
+			{
+				Qvv<V> out;
+				out.rotation = quat_mul(fp, lhs.rotation, rhs.rotation);
+				Vec3<V> scaled;
+				scaled.x = fp.mul(lhs.translation.x, rhs.scale.x);
+				scaled.y = fp.mul(lhs.translation.y, rhs.scale.y);
+				scaled.z = fp.mul(lhs.translation.z, rhs.scale.z);
+				const Vec3<V> rotated = quat_mul_vector3(fp, scaled, rhs.rotation);
+				out.translation.x = fp.add(rotated.x, rhs.translation.x);
+				out.translation.y = fp.add(rotated.y, rhs.translation.y);
+				out.translation.z = fp.add(rotated.z, rhs.translation.z);
+				out.scale.x = fp.mul(lhs.scale.x, rhs.scale.x);
+				out.scale.y = fp.mul(lhs.scale.y, rhs.scale.y);
+				out.scale.z = fp.mul(lhs.scale.z, rhs.scale.z);
+				return out;
+			}
+
+			// which branch rtm::qvv_mul takes: vector_any_less_than3(vector_min(lhs.scale, rhs.scale), 0), qvvf.h:317-320 (either stream of a pair)
+			template<class V>
+			__device__ __forceinline__ bool takes_negative_branch(const Fp<V>& fp, const Vec3<V>& lhs_scale, const Vec3<V>& rhs_scale)
+			{
+				return fp.any_negative(lhs_scale.x, rhs_scale.x) || fp.any_negative(lhs_scale.y, rhs_scale.y) || fp.any_negative(lhs_scale.z, rhs_scale.z);
+			}
+
+			// ---- qvvf_matrix3x4f_transform_error_metric (transform_error_metrics.h:389-464): the same walk on 3x4 matrices. Every operation is an
+			// IEEE mul / add / sqrt: this metric is bit-identical to the reference on any CPU ----
+			template<class V> struct Mat34 { V m[4][3]; };		// rows: x_axis, y_axis, z_axis, w_axis (translation)
+
+			// rtm::matrix_from_qvv, matrix3x4f.h:134-159 (convert_transforms :397-413)
+			template<class V>
+			__device__ __forceinline__ Mat34<V> matrix_from_qvv(const Fp<V>& fp, const Qvv<V>& q)
+			{
+				const V x2 = fp.add(q.rotation.x, q.rotation.x), y2 = fp.add(q.rotation.y, q.rotation.y), z2 = fp.add(q.rotation.z, q.rotation.z);
+				const V xx = fp.mul(q.rotation.x, x2), xy = fp.mul(q.rotation.x, y2), xz = fp.mul(q.rotation.x, z2);
+				const V yy = fp.mul(q.rotation.y, y2), yz = fp.mul(q.rotation.y, z2), zz = fp.mul(q.rotation.z, z2);
+				const V wx = fp.mul(q.rotation.w, x2), wy = fp.mul(q.rotation.w, y2), wz = fp.mul(q.rotation.w, z2);
+				const V one = fp.splat(1.0f);
+				Mat34<V> out;
+				out.m[0][0] = fp.mul(fp.sub(one, fp.add(yy, zz)), q.scale.x);	out.m[0][1] = fp.mul(fp.add(xy, wz), q.scale.x);				out.m[0][2] = fp.mul(fp.sub(xz, wy), q.scale.x);
+				out.m[1][0] = fp.mul(fp.sub(xy, wz), q.scale.y);				out.m[1][1] = fp.mul(fp.sub(one, fp.add(xx, zz)), q.scale.y);	out.m[1][2] = fp.mul(fp.add(yz, wx), q.scale.y);
+				out.m[2][0] = fp.mul(fp.add(xz, wy), q.scale.z);				out.m[2][1] = fp.mul(fp.sub(yz, wx), q.scale.z);				out.m[2][2] = fp.mul(fp.sub(one, fp.add(xx, yy)), q.scale.z);
+				out.m[3][0] = q.translation.x;									out.m[3][1] = q.translation.y;									out.m[3][2] = q.translation.z;
+				return out;
+			}
+
+			// rtm::matrix_mul(lhs, rhs), matrix3x4f.h:298-321 (local_to_object_space :415-436)
+			template<class V>
+			__device__ __forceinline__ Mat34<V> matrix_mul(const Fp<V>& fp, const Mat34<V>& l, const Mat34<V>& r)
+			{
+				Mat34<V> out;
+				#pragma unroll
+				for (int row = 0; row < 4; ++row)
+					#pragma unroll
+					for (int c = 0; c < 3; ++c)
+					{
+						V tmp = fp.mul(l.m[row][0], r.m[0][c]);
+						tmp = fp.add(fp.mul(l.m[row][1], r.m[1][c]), tmp);
+						tmp = fp.add(fp.mul(l.m[row][2], r.m[2][c]), tmp);
+						out.m[row][c] = row == 3 ? fp.add(r.m[3][c], tmp) : tmp;
+					}
+				return out;
+			}
+
+			template<class V>
+			__device__ __forceinline__ void store_matrix_planes(V* planes, uint32_t plane_stride, uint32_t bone, const Mat34<V>& q)
+			{
+				#pragma unroll
+				for (int row = 0; row < 4; ++row)
+					#pragma unroll
+					for (int c = 0; c < 3; ++c)
+						planes[(row * 3 + c) * plane_stride + bone] = q.m[row][c];
+			}
+
+			template<class V>
+			__device__ __forceinline__ Mat34<V> load_matrix_planes(const V* planes, uint32_t plane_stride, uint32_t bone)
+			{
+				Mat34<V> q;
+				#pragma unroll
+				for (int row = 0; row < 4; ++row)
+					#pragma unroll
+					for (int c = 0; c < 3; ++c)
+						q.m[row][c] = planes[(row * 3 + c) * plane_stride + bone];
+				return q;
+			}
+
+			// object transforms of a warp's pose in shared memory: [component][bone] planes of V (32 lanes reading 32 different parents hit
+			// different banks; a float2 plane element is one 8 byte access)
+			template<class V>
+			__device__ __forceinline__ void store_planes(V* planes, uint32_t plane_stride, uint32_t bone, const Qvv<V>& q)
+			{
+				planes[0 * plane_stride + bone] = q.rotation.x;
+				planes[1 * plane_stride + bone] = q.rotation.y;
+				planes[2 * plane_stride + bone] = q.rotation.z;
+				planes[3 * plane_stride + bone] = q.rotation.w;
+				planes[4 * plane_stride + bone] = q.translation.x;
+				planes[5 * plane_stride + bone] = q.translation.y;
+				planes[6 * plane_stride + bone] = q.translation.z;
+				planes[7 * plane_stride + bone] = q.scale.x;
+				planes[8 * plane_stride + bone] = q.scale.y;
+				planes[9 * plane_stride + bone] = q.scale.z;
+			}
+
+			template<class V>
+			__device__ __forceinline__ Qvv<V> load_planes(const V* planes, uint32_t plane_stride, uint32_t bone)
+			{
+				Qvv<V> q;
+				q.rotation.x = planes[0 * plane_stride + bone];
+				q.rotation.y = planes[1 * plane_stride + bone];
+				q.rotation.z = planes[2 * plane_stride + bone];
+				q.rotation.w = planes[3 * plane_stride + bone];
+				q.translation.x = planes[4 * plane_stride + bone];
+				q.translation.y = planes[5 * plane_stride + bone];
+				q.translation.z = planes[6 * plane_stride + bone];
+				q.scale.x = planes[7 * plane_stride + bone];
+				q.scale.y = planes[8 * plane_stride + bone];
+				q.scale.z = planes[9 * plane_stride + bone];
+				return q;
+			}
+
+			// ---- the out of line paths: a bone whose qvv_mul takes the negative scale branch in either stream. They work on the planes in
+			// shared memory, stream by stream on plain floats, so that the packed registers of the fast path never meet a conditional
+			// assignment (a packed value that is conditionally modified gets split into its halves and re-paired with moves) ----
+			template<class V> struct Streams;
+			template<> struct Streams<float> { static constexpr int count = 1; };
+			template<> struct Streams<float2> { static constexpr int count = 2; };
+
+			template<class V>
+			__device__ __forceinline__ Qvv<float> read_stream(const V* planes, uint32_t plane_stride, uint32_t bone, int stream)
+			{
+				const float* words = reinterpret_cast<const float*>(planes);
+				const auto at = [&](uint32_t component) { return words[(size_t(component) * plane_stride + bone) * Streams<V>::count + stream]; };
+				Qvv<float> q;
+				q.rotation = Quat<float>{ at(0), at(1), at(2), at(3) };
+				q.translation = Vec3<float>{ at(4), at(5), at(6) };
+				q.scale = Vec3<float>{ at(7), at(8), at(9) };
+				return q;
+			}
+
+			template<class V>
+			__device__ __forceinline__ void write_stream(V* planes, uint32_t plane_stride, uint32_t bone, int stream, const Qvv<float>& q)
+			{
+				float* words = reinterpret_cast<float*>(planes);
+				const auto put = [&](uint32_t component, float value) { words[(size_t(component) * plane_stride + bone) * Streams<V>::count + stream] = value; };
+				put(0, q.rotation.x); put(1, q.rotation.y); put(2, q.rotation.z); put(3, q.rotation.w);
+				put(4, q.translation.x); put(5, q.translation.y); put(6, q.translation.z);
+				put(7, q.scale.x); put(8, q.scale.y); put(9, q.scale.z);
+			}
+
+			// rtm::qvv_mul on one stream, whichever branch it takes
+			__device__ __forceinline__ Qvv<float> qvv_mul_any(const Qvv<float>& lhs, const Qvv<float>& rhs)
+			{
+				const Fp<float> fp{};
+				if (!takes_negative_branch(fp, lhs.scale, rhs.scale))
+					return qvv_mul_positive(fp, lhs, rhs);
+				Qvv<float> out;
+				qvv_mul_negative_scale(&lhs, &rhs, &out);
+				return out;
+			}
+
+			// planes[bone] = qvv_normalize(qvv_mul(planes[bone] (the local transform), planes[parent])), every stream
+			template<class V>
+			__device__ __noinline__ void object_transform_slow(V* planes, uint32_t plane_stride, uint32_t bone, uint32_t parent)
+			{
+				const Fp<float> fp{};
+				for (int stream = 0; stream < Streams<V>::count; ++stream)
+				{
+					Qvv<float> out = qvv_mul_any(read_stream(planes, plane_stride, bone, stream), read_stream(planes, plane_stride, parent, stream));
+					out.rotation = quat_normalize(fp, out.rotation);
+					write_stream(planes, plane_stride, bone, stream, out);
+				}
+			}
+
+			// A parent that does not precede its child: the reference would read an object transform it has not written yet. Reported, and
+			// the bone is treated as a root.
+			__device__ __forceinline__ bool parent_follows(bool active, uint32_t bone, uint32_t parent)
+			{
+				return active && parent != k_invalid_track && parent >= bone;
+			}
+
+			// The hierarchy walk of one chunk of 32 bones (bone = base + lane), in wavefronts: `compute()` runs on a lane once its parent's
+			// object transform is final. Every lane of the warp calls it; roots and inactive lanes never compute.
+			template<class Compute>
+			__device__ __forceinline__ void wavefront_walk(bool active, uint32_t parent, uint32_t base, Compute&& compute)
+			{
+				bool pending = active && parent != k_invalid_track;
+				uint32_t done_mask = __ballot_sync(0xFFFFFFFFu, active && !pending);
+				while (__any_sync(0xFFFFFFFFu, pending))
+				{
+					const bool ready = pending && (parent < base || ((done_mask >> (parent - base)) & 1u) != 0);
+					if (ready)
+					{
+						compute();
+						pending = false;
+					}
+					__syncwarp();
+					done_mask |= __ballot_sync(0xFFFFFFFFu, ready);
+				}
+			}
+
+			// ---- the walk on 48 byte pose rows in shared memory (the object space decode): a bone's row holds its local rtm::qvvf (rotation
+			// xyzw, translation xyz + 0, scale xyz + 0) and is overwritten in place by its object transform, as a qvvf row of the same layout
+			// or as the xyz lanes of the matrix's x_axis, y_axis, z_axis, w_axis. A lane moves its own row with three 16 byte accesses: rows
+			// are 48 bytes apart, so the 8 lanes of each quarter warp cover the 32 banks exactly once (no conflict) ----
+			__device__ __forceinline__ Qvv<float> load_qvv_row(const float4* row)
+			{
+				const float4 r = row[0], t = row[1], s = row[2];
+				Qvv<float> q;
+				q.rotation = Quat<float>{ r.x, r.y, r.z, r.w };
+				q.translation = Vec3<float>{ t.x, t.y, t.z };
+				q.scale = Vec3<float>{ s.x, s.y, s.z };
+				return q;
+			}
+
+			__device__ __forceinline__ void store_qvv_row(float4* row, const Qvv<float>& q)
+			{
+				row[0] = make_float4(q.rotation.x, q.rotation.y, q.rotation.z, q.rotation.w);
+				row[1] = make_float4(q.translation.x, q.translation.y, q.translation.z, 0.0f);
+				row[2] = make_float4(q.scale.x, q.scale.y, q.scale.z, 0.0f);
+			}
+
+			__device__ __forceinline__ Mat34<float> load_matrix_row(const float4* row)
+			{
+				const float4 a = row[0], b = row[1], c = row[2];
+				return Mat34<float>{ { { a.x, a.y, a.z }, { a.w, b.x, b.y }, { b.z, b.w, c.x }, { c.y, c.z, c.w } } };
+			}
+
+			__device__ __forceinline__ void store_matrix_row(float4* row, const Mat34<float>& m)
+			{
+				row[0] = make_float4(m.m[0][0], m.m[0][1], m.m[0][2], m.m[1][0]);
+				row[1] = make_float4(m.m[1][1], m.m[1][2], m.m[2][0], m.m[2][1]);
+				row[2] = make_float4(m.m[2][2], m.m[3][0], m.m[3][1], m.m[3][2]);
+			}
+
+			// row = qvv_normalize(qvv_mul(row (the local transform), parent_row)) through whichever branch qvv_mul takes
+			__device__ __noinline__ void object_row_slow(float4* row, const float4* parent_row)
+			{
+				const Fp<float> fp{};
+				Qvv<float> out = qvv_mul_any(load_qvv_row(row), load_qvv_row(parent_row));
+				out.rotation = quat_normalize(fp, out.rotation);
+				store_qvv_row(row, out);
+			}
+
+			// One warp takes the pose at `pose` (num_tracks rows of 48 bytes in shared memory) to object space with the skeleton `parents`:
+			// qvvf_transform_error_metric::local_to_object_space (transform_error_metrics.h:289-310) or, MATRIX, convert_transforms +
+			// local_to_object_space of qvvf_matrix3x4f_transform_error_metric (:397-436). Every lane of the warp calls it; returns the lane's
+			// ACLB200_ERROR_FLAG_* bits.
+			__device__ __forceinline__ uint32_t pose_rows_to_object_space(uint8_t* pose, uint32_t num_tracks, const uint32_t* parents, bool matrix)
+			{
+				const Fp<float> fp{};
+				const uint32_t lane = threadIdx.x & 31u;
+				uint32_t flags = 0;
+				for (uint32_t base = 0; base < num_tracks; base += 32)
+				{
+					const uint32_t bone = base + lane;
+					const bool active = bone < num_tracks;
+					uint32_t parent = active ? __ldg(parents + bone) : k_invalid_track;
+					if (parent_follows(active, bone, parent))
+					{
+						flags |= ACLB200_ERROR_FLAG_INVALID_SKELETON;
+						parent = k_invalid_track;
+					}
+					float4* row = reinterpret_cast<float4*>(pose + size_t(bone) * 48);
+					if (matrix)
+					{
+						if (active)
+							store_matrix_row(row, matrix_from_qvv(fp, load_qvv_row(row)));		// convert_transforms
+						__syncwarp();
+						wavefront_walk(active, parent, base, [&]()
+						{
+							const float4* above = reinterpret_cast<const float4*>(pose + size_t(parent) * 48);
+							store_matrix_row(row, matrix_mul(fp, load_matrix_row(row), load_matrix_row(above)));
+						});
+					}
+					else
+					{
+						wavefront_walk(active, parent, base, [&]()
+						{
+							const float4* above = reinterpret_cast<const float4*>(pose + size_t(parent) * 48);
+							const Qvv<float> mine = load_qvv_row(row);
+							const Qvv<float> up = load_qvv_row(above);
+							if (takes_negative_branch(fp, mine.scale, up.scale))
+							{
+								flags |= ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
+								object_row_slow(row, above);
+							}
+							else
+							{
+								// rtm::qvv_normalize(rtm::qvv_mul(local, parent_object)), qvvf.h:426-430
+								Qvv<float> object = qvv_mul_positive(fp, mine, up);
+								object.rotation = quat_normalize(fp, object.rotation);
+								store_qvv_row(row, object);
+							}
+						});
+					}
+				}
+				return flags;
+			}
+		}
+	}
+}

@@ -403,6 +403,15 @@ namespace acl_b200
 			else
 				m_device->check(aclb200_scalar_decompress_track(m_device->get(), m_clipset, d_requests, d_track_indices, num_requests, &options, d_out, stream), "aclb200_scalar_decompress_track");
 		}
+		// decompress_tracks() + the hierarchy walk in one launch (aclb200_decompress_tracks_object_space): object space bones of 48 bytes,
+		// ACLB200_OBJECT_QVVF or ACLB200_OBJECT_MATRIX3X4F; clip c uses the skeleton at d_parent_indices + d_skeleton_offsets[c] (nullptr: 0)
+		void decompress_tracks_object_space(const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, void* d_out, uint32_t* d_out_flags = nullptr,
+			void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_object_space(m_device->get(), m_clipset, d_requests, num_requests, &options, d_parent_indices,
+				d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_object_space");
+		}
 		// host buffers in, host buffers out, synchronous
 		void decompress_tracks_host(const aclb200_request* requests, uint32_t num_requests, const aclb200_options& options, void* out, size_t out_bytes)
 		{

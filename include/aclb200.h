@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 5
+#define ACLB200_VERSION_MINOR 6
 
 typedef enum aclb200_status
 {
@@ -380,6 +380,37 @@ ACLB200_API aclb200_status aclb200_set_error_chunk_bytes(aclb200_context* contex
  * ACLB200_ERROR_FLAG_* met on the way. */
 ACLB200_API aclb200_status aclb200_local_to_object_space(aclb200_context* context, const void* d_local_poses, void* d_object_poses, uint64_t num_poses,
 	uint32_t num_tracks, uint64_t pose_stride_bytes, const uint32_t* d_parent_indices, uint32_t* d_out_flags, void* stream);
+
+/* What aclb200_decompress_tracks_object_space writes per bone (48 bytes either way) */
+enum
+{
+	ACLB200_OBJECT_QVVF = 0,		/* rtm::qvvf: rotation xyzw, translation xyz + 0, scale xyz + 0 (what aclb200_local_to_object_space writes) */
+	ACLB200_OBJECT_MATRIX3X4F = 1	/* rtm::matrix3x4f without its constant w lanes: x_axis xyz, y_axis xyz, z_axis xyz, w_axis xyz */
+};
+
+/* aclb200_decompress_tracks followed by the hierarchy walk, in one kernel: the local poses never leave shared memory. Request r computes
+ * what aclb200_decompress_tracks computes for it (same options, rounding, looping, per request policies, default modes and bind pose;
+ * a clip set whose bound database has chunks streamed in decodes from them) and takes the pose to object space with its clip's skeleton:
+ *   ACLB200_OBJECT_QVVF       qvvf_transform_error_metric::local_to_object_space (transform_error_metrics.h:289-310):
+ *                             obj = qvv_normalize(qvv_mul(local, obj[parent])), roots copied; byte for byte what
+ *                             aclb200_local_to_object_space writes for the decoded pose
+ *   ACLB200_OBJECT_MATRIX3X4F convert_transforms (matrix_from_qvv) + local_to_object_space of qvvf_matrix3x4f_transform_error_metric
+ *                             (:397-436): obj = matrix_mul(local, obj[parent]), roots copied; bit-identical to the reference on any CPU
+ * Every operation is IEEE and unfused; ACLB200_MATH_FAST is accepted and runs the exact decode.
+ *   d_parent_indices    device: parent of each bone (0xFFFFFFFF = root); clip c's skeleton starts at d_parent_indices + d_skeleton_offsets[c]
+ *   d_skeleton_offsets  device u32[num_clips], or NULL: every clip uses the skeleton at offset 0
+ *   d_out               pose r at d_out + r * options->pose_stride_bytes (0 = max_tracks * 48), 48 bytes per bone; stride and alignment
+ *                       as aclb200_decompress_tracks requires for ACLB200_LAYOUT_QVV48. A request with an invalid clip index writes
+ *                       nothing, and no byte past a clip's num_tracks * 48 is written.
+ *   d_out_flags         device uint32, optional: cleared, then ACLB200_ERROR_FLAG_* met on the way OR-ed in, as aclb200_local_to_object_space
+ *                       does (a parent that does not precede its child is reported and its bone treated as a root)
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, writing nothing: skip masks (options->skip_mask, d_skip_track_mask) or a `skipped` default mode
+ * (an object transform needs every sub-track of its parents), an output layout other than QVV48, an unknown object_kind, NULL parents, a
+ * scalar clip set. ACLB200_ERR_UNSUPPORTED when one pose does not fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_object_space(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
 
 /* Parity / debugging hooks (integer stages of the decode, bit-exact against the reference):
  *  - aclb200_debug_seek: the state seek_v0 computes, one aclb200_seek_state per request (device output).

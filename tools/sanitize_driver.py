@@ -1,12 +1,12 @@
 """Small workload for compute-sanitizer (tools/sanitize.sh): every kernel of the library once or twice, checked against the oracle --
 chained playback through the pipeline kernel (groups, tail crossing, base row reuse), ragged random requests, per track rounding,
-skipped defaults (plain kernels), decompress_track, the chained scalar kernel."""
+skipped defaults (plain kernels), decompress_track, the object space decode (both kinds, a skeleton per clip), the chained scalar kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 import acl_b200 as ab
-from oracle import port
+from oracle import object_space, port
 from tests import clips
 
 L = clips.DEFINED_LANES
@@ -49,6 +49,23 @@ tracks = torch.from_numpy(rng.integers(0, 17, len(req)).astype(np.uint32)).cuda(
 one = torch.zeros((len(req), 12), dtype=torch.float32, device="cuda")
 ctx.decompress_track(cs, d_req, tracks, len(req), ab.Options(), one)
 torch.cuda.synchronize()
+# object space decode: the OBJECT = true instances of the plain kernel, a binary tree skeleton per clip
+counts = [clips.TRANSFORM_SPECS[n].num_tracks for n in names]
+trees = [np.array([0xFFFFFFFF] + [(b - 1) // 2 for b in range(1, n)], np.uint32) for n in counts]
+d_parents = torch.from_numpy(np.concatenate(trees)).cuda()
+d_offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)[:-1]]).astype(np.uint32)).cuda()
+for kind in (ab.OBJECT_QVVF, ab.OBJECT_MATRIX3X4F):
+    out = torch.zeros((len(req), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+    ctx.decompress_tracks_object_space(cs, d_req, len(req), ab.Options(), d_parents, kind, out, d_skeleton_offsets=d_offsets)
+    torch.cuda.synchronize()
+    got = out.cpu().numpy()
+    for i in range(0, len(req), 7):
+        c = req_clip[i]
+        local = port.transform_decompress_tracks(blobs[c], settings, float(req_time[i]))
+        if kind == ab.OBJECT_MATRIX3X4F:
+            bad += not clips.bit_equal(got[i, :counts[c]], object_space.port_local_to_object_space_matrix(local, trees[c]))
+        else:
+            bad += not clips.bit_equal(got[i, :counts[c]][:, L], port.local_to_object_space(local, trees[c], port.NORMALIZE_IEEE)[:, L])
 # scalar clips
 for name in ("float1", "float3", "vector4", "float1_c4_small"):
     blob = clips.load_blob(name); spec = clips.SCALAR_SPECS[name]
