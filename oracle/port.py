@@ -130,6 +130,12 @@ def num_tracks_of(blob: np.ndarray) -> int:
     return int(blob[16:20].view(np.uint32)[0])
 
 
+def hash32(data: np.ndarray) -> int:
+    """hash32 (FNV-1a 32, core/hash.h) of a byte array: what compressed_tracks stores over bytes [8, size)."""
+    data = np.ascontiguousarray(data, dtype=np.uint8)
+    return int(lib().aclo_hash32(data.ctypes.data, data.size))
+
+
 def validate(blob: np.ndarray, check_hash: bool = False) -> int:
     return lib().aclo_validate(blob.ctypes.data, blob.size, int(check_hash))
 
