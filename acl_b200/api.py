@@ -159,6 +159,8 @@ def _lib():
         l.aclb200_decompress_all_samples.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp]
         l.aclb200_local_to_object_space.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp]
         l.aclb200_decompress_tracks_object_space.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, u32, vp, vp, vp]
+        l.aclb200_decompress_tracks_additive.argtypes = [vp, vp, vp, u32, C.POINTER(Options), u32, vp, vp, vp, u32, vp, vp, vp]
+        l.aclb200_apply_additive_to_base.argtypes = [vp, vp, vp, vp, u64, u32, u64, u32, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -185,7 +187,7 @@ def exported_symbols() -> list[str]:
         "aclb200_calculate_compression_error", "aclb200_set_error_chunk_bytes", "aclb200_local_to_object_space",
         "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
         "aclb200_database_get_loaded_chunks", "aclb200_database_stream_in", "aclb200_database_stream_out", "aclb200_clipset_bind_database",
-        "aclb200_decompress_tracks_object_space",
+        "aclb200_decompress_tracks_object_space", "aclb200_decompress_tracks_additive", "aclb200_apply_additive_to_base",
     ]
 
 
@@ -196,6 +198,20 @@ def make_requests(clips, times) -> np.ndarray:
     out = np.empty(clips.shape[0], dtype=REQUEST_DTYPE)
     out["clip"] = clips
     out["sample_time"] = times
+    return out
+
+
+ADDITIVE_REQUEST_DTYPE = np.dtype([("base_clip", np.uint32), ("base_time", np.float32), ("additive_clip", np.uint32), ("additive_time", np.float32)])
+
+
+def make_additive_requests(base_clips, base_times, additive_clips, additive_times) -> np.ndarray:
+    """(base clip, base time, additive clip, additive time) arrays -> aclb200_additive_request[]"""
+    base_clips = np.asarray(base_clips, dtype=np.uint32)
+    out = np.empty(base_clips.shape[0], dtype=ADDITIVE_REQUEST_DTYPE)
+    out["base_clip"] = base_clips
+    out["base_time"] = np.asarray(base_times, dtype=np.float32)
+    out["additive_clip"] = np.asarray(additive_clips, dtype=np.uint32)
+    out["additive_time"] = np.asarray(additive_times, dtype=np.float32)
     return out
 
 
@@ -384,6 +400,18 @@ class Context:
                                                                   C.byref(options), _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
                                                                   kind, _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
+    def decompress_tracks_additive(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, additive_format: int = 0,
+                                   d_clip_additive_formats=None, d_parent_indices=None, kind: int = 0, d_skeleton_offsets=None,
+                                   d_out_flags=None, stream=None) -> None:
+        """num_requests additive pairs (make_additive_requests): pose r = apply_additive_to_base(format, decode(base), decode(additive)), the
+        additive half with the track_writer defaults. format: d_clip_additive_formats[additive clip] (uint8, None: additive_format for
+        every pair). With d_parent_indices the combined pose leaves in object space as `kind` rows (OBJECT_*), the skeleton of the base
+        clip c at d_parent_indices + d_skeleton_offsets[c]; without, in options.output_layout. d_out_flags: optional uint32 ERROR_FLAG_*."""
+        self._check(_lib().aclb200_decompress_tracks_additive(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                              C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
+                                                              _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
+                                                              _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
     def decompress_track(self, clipset: ClipSet, d_requests, d_track_indices, num_requests: int, options: Options, d_out, stream=None) -> None:
         self._check(_lib().aclb200_decompress_track(self._handle, clipset._handle, _device_ptr(d_requests), _device_ptr(d_track_indices),
                                                     num_requests, C.byref(options), _device_ptr(d_out), _stream_ptr(stream)))
@@ -438,6 +466,13 @@ class Context:
         self._check(_lib().aclb200_local_to_object_space(self._handle, _device_ptr(d_local_poses), _device_ptr(d_object_poses), num_poses,
                                                          num_tracks, pose_stride_bytes, _device_ptr(d_parent_indices),
                                                          _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def apply_additive_to_base(self, d_base_poses, d_additive_poses, d_out, num_poses: int, num_tracks: int, additive_format: int,
+                               pose_stride_bytes: int = 0, d_out_flags=None, stream=None) -> None:
+        """acl::apply_additive_to_base on every bone of num_poses QVV48 poses; d_out may be either input."""
+        self._check(_lib().aclb200_apply_additive_to_base(self._handle, _device_ptr(d_base_poses), _device_ptr(d_additive_poses), _device_ptr(d_out),
+                                                          num_poses, num_tracks, pose_stride_bytes, additive_format, _device_ptr(d_out_flags),
+                                                          _stream_ptr(stream)))
 
     # ---- host buffers in, host buffers out (the call the C++ header shim uses) ----
     def decompress_tracks_host(self, clipset: ClipSet, requests: np.ndarray, options: Options, out: np.ndarray) -> np.ndarray:

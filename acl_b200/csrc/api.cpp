@@ -19,7 +19,7 @@ namespace aclb200
 
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			bool object_space = false)
+			bool object_space = false, bool additive_pairs = false)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -106,8 +106,10 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: an object transform needs every sub-track of its parents (no skip masks, no `skipped` default mode)");
 			if (object_space && options->output_layout != ACLB200_LAYOUT_QVV48)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: the output layout must be QVV48");
+			if (additive_pairs && (any_skipped || any_masked))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: apply_additive_to_base needs every sub-track of both poses (no skip masks, no `skipped` default mode)");
 			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database,
-				object_space);
+				object_space || additive_pairs, additive_pairs);
 			return ACLB200_OK;
 		}
 
@@ -126,7 +128,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.6 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.7 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -358,6 +360,79 @@ extern "C"
 		}
 		return finish_launch(context, launch_transform_decompress_tracks_object_space(params, params.db_tiers != nullptr, cuda_stream),
 			"decompress_tracks_object_space");
+	}
+
+	aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		if (num_requests > 0x7FFFFFFFu)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: more than 2^31 - 1 pairs");
+		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
+		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
+		DecodeParams params;
+		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, d_out,
+			true, false, params, false, true);
+		if (status != ACLB200_OK)
+			return status;
+		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: additive_format out of range");
+		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: unknown object_kind");
+		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: object space output needs the QVV48 layout");
+		// plan_launch kept both poses of a pair in shared memory and gave up key frame staging first: what is left must fit one block
+		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_additive: the two poses of a pair do not fit in a block's shared memory");
+		if (num_requests == 0)
+			return ACLB200_OK;
+		params.parent_indices = d_parent_indices;
+		params.skeleton_offsets = d_skeleton_offsets;
+		params.object_flags = d_out_flags;
+		params.object_kind = object_kind;
+		params.additive_format = additive_format;
+		params.clip_additive_formats = d_clip_additive_formats;
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		if (d_out_flags != nullptr)
+		{
+			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
+			if (cleared != cudaSuccess)
+				return check_cuda(context, cleared, "decompress_tracks_additive");
+		}
+		return finish_launch(context, launch_transform_decompress_tracks_additive(params, params.db_tiers != nullptr, cuda_stream),
+			"decompress_tracks_additive");
+	}
+
+	aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
+		void* d_out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, uint32_t additive_format,
+		uint32_t* d_out_flags, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: additive_format out of range");
+		if (num_poses == 0 || num_tracks == 0)
+			return ACLB200_OK;
+		if (d_base_poses == nullptr || d_additive_poses == nullptr || d_out == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: null pose pointer");
+		const uint64_t stride = pose_stride_bytes != 0 ? pose_stride_bytes : uint64_t(num_tracks) * 48;
+		if (stride < uint64_t(num_tracks) * 48 || (stride % 16) != 0
+			|| ((reinterpret_cast<uintptr_t>(d_base_poses) | reinterpret_cast<uintptr_t>(d_additive_poses) | reinterpret_cast<uintptr_t>(d_out)) % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		if (d_out_flags != nullptr)
+		{
+			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
+			if (cleared != cudaSuccess)
+				return check_cuda(context, cleared, "apply_additive_to_base");
+		}
+		return finish_launch(context, launch_apply_additive(static_cast<const uint8_t*>(d_base_poses), static_cast<const uint8_t*>(d_additive_poses),
+			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, additive_format, d_out_flags, context->num_sms, cuda_stream),
+			"apply_additive_to_base");
 	}
 
 	aclb200_status aclb200_decompress_track(aclb200_context* context, const aclb200_clipset* clipset,

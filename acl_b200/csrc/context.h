@@ -179,17 +179,25 @@ namespace aclb200
 		const uint32_t* skeleton_offsets;			// [num_clips] first parent index of each clip's skeleton, or nullptr (every clip at 0)
 		uint32_t* object_flags;						// ACLB200_ERROR_FLAG_* are OR-ed in, or nullptr
 		uint32_t object_kind;						// ACLB200_OBJECT_*
+		// the additive decode (aclb200_decompress_tracks_additive): requests 2r / 2r + 1 are the base / additive halves of pair r, output r;
+		// parent_indices == nullptr there keeps the combined poses in local space
+		const uint8_t* clip_additive_formats;		// [num_clips] acl::additive_clip_format8 per additive clip (above 3: none), or nullptr
+		uint32_t additive_format;					// the format when clip_additive_formats == nullptr
 	};
 
 	// kernels.cu
+	// additive_pairs: the additive decode, planned in whole pairs with both poses of a pair in shared memory
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false,
-		bool force_output_staging = false);
+		bool force_output_staging = false, bool additive_pairs = false);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);
 	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_tracks_object_space(const DecodeParams& params, bool database, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream);
+	cudaError_t launch_apply_additive(const uint8_t* base_poses, const uint8_t* additive_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
+		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);
 	cudaError_t launch_transform_debug_unpack(const DecodeParams& params, uint32_t* d_out, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);

@@ -1,6 +1,7 @@
 // acl_b200/csrc/object_space.cuh -- the hierarchy walk shared by the error measurement (error_metric.cu: object_space_kernel) and the
 // object space decode (kernels.cu: transform_decompress_tracks_kernel<..., OBJECT = true>): the reference's qvv and 3x4 matrix operations
-// restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose.
+// restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which the
+// error measurement, the additive decode (ADDITIVE = true) and aclb200_apply_additive_to_base share.
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
@@ -215,6 +216,35 @@ namespace aclb200
 			__device__ __forceinline__ bool takes_negative_branch(const Fp<V>& fp, const Vec3<V>& lhs_scale, const Vec3<V>& rhs_scale)
 			{
 				return fp.any_negative(lhs_scale.x, rhs_scale.x) || fp.any_negative(lhs_scale.y, rhs_scale.y) || fp.any_negative(lhs_scale.z, rhs_scale.z);
+			}
+
+			// acl::apply_additive_to_base(format, base, additive), includes/acl/core/additive_utils.h:131-167 (format = additive_clip_format8:
+			// 1 relative = qvv_mul(additive, base), 2 additive0, 3 additive1; transform_add0 / transform_add1 :131-145), positive scales.
+			// Format 0 (none) is the caller's business: it returns the additive transform unchanged.
+			template<class V>
+			__device__ __forceinline__ Qvv<V> apply_additive_to_base_positive(const Fp<V>& fp, uint32_t format, const Qvv<V>& base, const Qvv<V>& additive)
+			{
+				if (format == 1)
+					return qvv_mul_positive(fp, additive, base);
+				Qvv<V> out;
+				out.rotation = quat_mul(fp, additive.rotation, base.rotation);
+				out.translation.x = fp.add(additive.translation.x, base.translation.x);
+				out.translation.y = fp.add(additive.translation.y, base.translation.y);
+				out.translation.z = fp.add(additive.translation.z, base.translation.z);
+				if (format == 2)
+				{
+					out.scale.x = fp.mul(additive.scale.x, base.scale.x);
+					out.scale.y = fp.mul(additive.scale.y, base.scale.y);
+					out.scale.z = fp.mul(additive.scale.z, base.scale.z);
+				}
+				else
+				{
+					const V one = fp.splat(1.0f);
+					out.scale.x = fp.mul(fp.add(one, additive.scale.x), base.scale.x);
+					out.scale.y = fp.mul(fp.add(one, additive.scale.y), base.scale.y);
+					out.scale.z = fp.mul(fp.add(one, additive.scale.z), base.scale.z);
+				}
+				return out;
 			}
 
 			// ---- qvvf_matrix3x4f_transform_error_metric (transform_error_metrics.h:389-464): the same walk on 3x4 matrices. Every operation is an
@@ -489,6 +519,64 @@ namespace aclb200
 					}
 				}
 				return flags;
+			}
+
+			// ---- apply_additive_to_base on pose rows (the additive decode and aclb200_apply_additive_to_base): one thread per bone, a row of 48
+			// bytes (QVV48: rotation xyzw, translation xyz + 0, scale xyz + 0, 16 byte aligned) or 40 bytes (QVV40: rotation xyzw, translation
+			// xyz, scale xyz, 8 byte aligned) ----
+			__device__ __forceinline__ Qvv<float> load_pose_row(const uint8_t* row, bool qvv40)
+			{
+				if (!qvv40)
+					return load_qvv_row(reinterpret_cast<const float4*>(row));
+				const float2* r = reinterpret_cast<const float2*>(row);
+				const float2 a = r[0], b = r[1], c = r[2], d = r[3], e = r[4];
+				Qvv<float> q;
+				q.rotation = Quat<float>{ a.x, a.y, b.x, b.y };
+				q.translation = Vec3<float>{ c.x, c.y, d.x };
+				q.scale = Vec3<float>{ d.y, e.x, e.y };
+				return q;
+			}
+
+			__device__ __forceinline__ void store_pose_row(uint8_t* row, const Qvv<float>& q, bool qvv40)
+			{
+				if (!qvv40)
+				{
+					store_qvv_row(reinterpret_cast<float4*>(row), q);
+					return;
+				}
+				float2* r = reinterpret_cast<float2*>(row);
+				r[0] = make_float2(q.rotation.x, q.rotation.y);
+				r[1] = make_float2(q.rotation.z, q.rotation.w);
+				r[2] = make_float2(q.translation.x, q.translation.y);
+				r[3] = make_float2(q.translation.z, q.scale.x);
+				r[4] = make_float2(q.scale.y, q.scale.z);
+			}
+
+			// out_row = rtm::qvv_mul(additive_row, base_row) through the matrix branch (a mirrored bone of a `relative` clip)
+			__device__ __noinline__ void additive_relative_row_slow(uint8_t* out_row, const uint8_t* base_row, const uint8_t* additive_row, bool qvv40)
+			{
+				const Qvv<float> base = load_pose_row(base_row, qvv40);
+				const Qvv<float> additive = load_pose_row(additive_row, qvv40);
+				Qvv<float> out;
+				qvv_mul_negative_scale(&additive, &base, &out);
+				store_pose_row(out_row, out, qvv40);
+			}
+
+			// out_row = acl::apply_additive_to_base(format, base_row, additive_row) (additive_utils.h:152-162; format 0 = none, the additive
+			// row itself). out_row may be either input. Returns ACLB200_ERROR_FLAG_NEGATIVE_SCALE when `relative` took qvv_mul's matrix branch.
+			__device__ __forceinline__ uint32_t apply_additive_row(uint8_t* out_row, const uint8_t* base_row, const uint8_t* additive_row, uint32_t format,
+				bool qvv40)
+			{
+				const Fp<float> fp{};
+				const Qvv<float> base = load_pose_row(base_row, qvv40);
+				const Qvv<float> additive = load_pose_row(additive_row, qvv40);
+				if (format == 1 && takes_negative_branch(fp, additive.scale, base.scale))
+				{
+					additive_relative_row_slow(out_row, base_row, additive_row, qvv40);
+					return ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
+				}
+				store_pose_row(out_row, format == 0 ? additive : apply_additive_to_base_positive(fp, format, base, additive), qvv40);
+				return 0;
 			}
 		}
 	}

@@ -412,6 +412,23 @@ namespace acl_b200
 			m_device->check(aclb200_decompress_tracks_object_space(m_device->get(), m_clipset, d_requests, num_requests, &options, d_parent_indices,
 				d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_object_space");
 		}
+		// decompress base + decompress additive (track_writer defaults) + acl::apply_additive_to_base per bone, in one launch
+		// (aclb200_decompress_tracks_additive). Format: d_clip_additive_formats[additive clip] (nullptr: additive_format). With parents the
+		// combined pose leaves in object space as object_kind rows (the base clip's skeleton), else as local rows in options.output_layout.
+		void decompress_tracks_additive(const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			uint32_t additive_format, const uint8_t* d_clip_additive_formats, void* d_out, const uint32_t* d_parent_indices = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_additive(m_device->get(), m_clipset, d_requests, num_requests, &options, additive_format,
+				d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_additive");
+		}
+		// acl::apply_additive_to_base over num_poses QVV48 poses already on the device (aclb200_apply_additive_to_base); d_out may be either input
+		void apply_additive_to_base(const void* d_base_poses, const void* d_additive_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks,
+			uint32_t additive_format, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_apply_additive_to_base(m_device->get(), d_base_poses, d_additive_poses, d_out, num_poses, num_tracks, pose_stride_bytes,
+				additive_format, d_out_flags, stream), "aclb200_apply_additive_to_base");
+		}
 		// host buffers in, host buffers out, synchronous
 		void decompress_tracks_host(const aclb200_request* requests, uint32_t num_requests, const aclb200_options& options, void* out, size_t out_bytes)
 		{

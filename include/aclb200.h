@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 6
+#define ACLB200_VERSION_MINOR 7
 
 typedef enum aclb200_status
 {
@@ -411,6 +411,53 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_object_space(aclb200_contex
 	const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* acl::additive_clip_format8 (core/additive_utils.h:42-66): how an additive clip applies to its base */
+enum { ACLB200_ADDITIVE_NONE = 0, ACLB200_ADDITIVE_RELATIVE = 1, ACLB200_ADDITIVE_ADDITIVE0 = 2, ACLB200_ADDITIVE_ADDITIVE1 = 3 };
+
+/* One layered pose: an additive clip sampled on top of a base clip. Both clips live in the same clip set; the two sample times are
+ * independent (keeping them in sync is the caller's business). */
+typedef struct aclb200_additive_request
+{
+	aclb200_request base;			/* the base clip and its sample time */
+	aclb200_request additive;		/* the additive clip and its sample time */
+} aclb200_additive_request;
+
+/* decompress base + decompress additive + acl::apply_additive_to_base (core/additive_utils.h:152-162) per bone, in one kernel: neither
+ * pose leaves shared memory. For pair r:
+ *   base pose      what aclb200_decompress_tracks computes for requests[r].base with `options` (rounding, looping, per request policies
+ *                  -- d_request_policies[r] applies to both halves --, per track rounding, normalisation, default modes and bind pose, a
+ *                  bound database's streamed tiers)
+ *   additive pose  the same for requests[r].additive, except that its default sub-tracks take the acl::track_writer defaults
+ *                  (track_writer.h:160-176): identity rotation, zero translation, the clip's own default scale (0 for additive1 clips)
+ *   format         d_clip_additive_formats[requests[r].additive.clip] (a byte above 3 reads as none) when that pointer is not NULL,
+ *                  else additive_format: none = the additive pose, relative = rtm::qvv_mul(additive, base) (its matrix branch for
+ *                  negative scales included), additive0 / additive1 = transform_add0 / transform_add1 (additive_utils.h:131-145)
+ *   d_out          d_parent_indices == NULL: the combined local pose in options->output_layout at d_out + r * options->pose_stride_bytes
+ *                  (0 = max_tracks * bone size). d_parent_indices given: the combined pose goes through the hierarchy walk of
+ *                  aclb200_decompress_tracks_object_space with the skeleton d_parent_indices + d_skeleton_offsets[requests[r].base.clip]
+ *                  (d_skeleton_offsets NULL: 0) and leaves as object_kind rows (QVV48 only).
+ *                  A pair with an invalid clip index on either side, or with clips of different track counts, writes nothing; no byte
+ *                  past a clip's num_tracks bones is written.
+ *   d_out_flags    device uint32, optional: cleared, then ACLB200_ERROR_FLAG_NEGATIVE_SCALE (a relative bone or the walk took qvv_mul's
+ *                  matrix branch) and ACLB200_ERROR_FLAG_INVALID_SKELETON OR-ed in
+ * Every operation is IEEE and unfused; ACLB200_MATH_FAST is accepted and runs the exact decode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, writing nothing: skip masks, a `skipped` default mode, additive_format > 3, a scalar clip
+ * set, an output that breaks the alignment rules of aclb200_decompress_tracks, and with parents an unknown object_kind or QVV40.
+ * ACLB200_ERR_UNSUPPORTED when the two poses of a pair do not fit in one block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* acl::apply_additive_to_base(additive_format, base, additive) on every bone of num_poses poses of rtm::qvvf rows (48 byte bones, 16 byte
+ * aligned; pose p of each buffer at p * pose_stride_bytes, 0 = num_tracks * 48): for a base pose that does not come from one clip (a
+ * blend). d_out may be either input. The translation and scale w lanes are written as 0. d_out_flags as aclb200_decompress_tracks_additive.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT: NULL pointers, additive_format > 3, misaligned rows. */
+ACLB200_API aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
+	void* d_out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, uint32_t additive_format,
+	uint32_t* d_out_flags, void* stream);
 
 /* Parity / debugging hooks (integer stages of the decode, bit-exact against the reference):
  *  - aclb200_debug_seek: the state seek_v0 computes, one aclb200_seek_state per request (device output).

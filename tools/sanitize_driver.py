@@ -1,6 +1,7 @@
 """Small workload for compute-sanitizer (tools/sanitize.sh): every kernel of the library once or twice, checked against the oracle --
 chained playback through the pipeline kernel (groups, tail crossing, base row reuse), ragged random requests, per track rounding,
-skipped defaults (plain kernels), decompress_track, the object space decode (both kinds, a skeleton per clip), the chained scalar kernel."""
+skipped defaults (plain kernels), decompress_track, the object space decode (both kinds, a skeleton per clip), the additive decode (local and
+object space, per clip formats) and aclb200_apply_additive_to_base, the chained scalar kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -66,6 +67,30 @@ for kind in (ab.OBJECT_QVVF, ab.OBJECT_MATRIX3X4F):
             bad += not clips.bit_equal(got[i, :counts[c]], object_space.port_local_to_object_space_matrix(local, trees[c]))
         else:
             bad += not clips.bit_equal(got[i, :counts[c]][:, L], port.local_to_object_space(local, trees[c], port.NORMALIZE_IEEE)[:, L])
+# additive decode: the ADDITIVE = true instances (pairs of clips with equal bone counts, every format, local then object space) and the
+# standalone apply_additive_kernel, in place
+pair_clip = np.array([c for c in range(len(names)) for _ in range(8)], np.uint32)
+pair_time = rng.uniform(-0.1, 2.5, (len(pair_clip), 2)).astype(np.float32)
+pairs = ab.make_additive_requests(pair_clip, pair_time[:, 0], pair_clip, pair_time[:, 1])
+d_pairs = torch.from_numpy(pairs.view(np.uint8)).cuda()
+d_formats = torch.from_numpy(np.arange(len(names), dtype=np.uint8) % 5).cuda()
+writer = port.settings_for_kind(0, constant_defaults=np.array([0, 0, 0, 1, 0, 0, 0, 0, 1, 1, 1, 0], np.float32))
+for parents in (None, d_parents):
+    out = torch.zeros((len(pairs), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+    ctx.decompress_tracks_additive(cs, d_pairs, len(pairs), ab.Options(), out, d_clip_additive_formats=d_formats, d_parent_indices=parents,
+                                   d_skeleton_offsets=d_offsets)
+    torch.cuda.synchronize()
+    got = out.cpu().numpy()
+    for i in range(0, len(pairs), 5):
+        c = pair_clip[i]
+        base = port.transform_decompress_tracks(blobs[c], settings, float(pair_time[i, 0]))
+        additive = port.transform_decompress_tracks(blobs[c], writer, float(pair_time[i, 1]))
+        want = port.apply_additive_to_base(int(c % 5) if c % 5 <= 3 else 0, base, additive, port.NORMALIZE_IEEE)
+        if parents is not None:
+            want = port.local_to_object_space(want, trees[c], port.NORMALIZE_IEEE)
+        bad += not clips.bit_equal(got[i, :counts[c]][:, L], want[:, L])
+ctx.apply_additive_to_base(out, out, out, len(pairs), cs.max_tracks, ab.ADDITIVE_ADDITIVE0)
+torch.cuda.synchronize()
 # scalar clips
 for name in ("float1", "float3", "vector4", "float1_c4_small"):
     blob = clips.load_blob(name); spec = clips.SCALAR_SPECS[name]
