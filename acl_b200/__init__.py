@@ -16,4 +16,5 @@ from .api import (  # noqa: F401
     ERROR_JOB_DTYPE, TRACK_ERROR_DTYPE, ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON,
     OBJECT_QVVF, OBJECT_MATRIX3X4F,
     ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1, ADDITIVE_REQUEST_DTYPE, make_additive_requests,
+    BLEND_REQUEST_DTYPE, make_blend_requests,
 )

@@ -161,6 +161,8 @@ def _lib():
         l.aclb200_decompress_tracks_object_space.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, u32, vp, vp, vp]
         l.aclb200_decompress_tracks_additive.argtypes = [vp, vp, vp, u32, C.POINTER(Options), u32, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_apply_additive_to_base.argtypes = [vp, vp, vp, vp, u64, u32, u64, u32, vp, vp]
+        l.aclb200_decompress_tracks_blend.argtypes = [vp, vp, vp, u32, C.POINTER(Options), C.c_float, vp, vp, vp, u32, vp, vp, vp]
+        l.aclb200_blend_poses.argtypes = [vp, vp, vp, vp, u64, u32, u64, C.c_float, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -188,6 +190,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
         "aclb200_database_get_loaded_chunks", "aclb200_database_stream_in", "aclb200_database_stream_out", "aclb200_clipset_bind_database",
         "aclb200_decompress_tracks_object_space", "aclb200_decompress_tracks_additive", "aclb200_apply_additive_to_base",
+        "aclb200_decompress_tracks_blend", "aclb200_blend_poses",
     ]
 
 
@@ -212,6 +215,20 @@ def make_additive_requests(base_clips, base_times, additive_clips, additive_time
     out["base_time"] = np.asarray(base_times, dtype=np.float32)
     out["additive_clip"] = np.asarray(additive_clips, dtype=np.uint32)
     out["additive_time"] = np.asarray(additive_times, dtype=np.float32)
+    return out
+
+
+BLEND_REQUEST_DTYPE = np.dtype([("from_clip", np.uint32), ("from_time", np.float32), ("to_clip", np.uint32), ("to_time", np.float32)])
+
+
+def make_blend_requests(from_clips, from_times, to_clips, to_times) -> np.ndarray:
+    """(from clip, from time, to clip, to time) arrays -> aclb200_blend_request[]"""
+    from_clips = np.asarray(from_clips, dtype=np.uint32)
+    out = np.empty(from_clips.shape[0], dtype=BLEND_REQUEST_DTYPE)
+    out["from_clip"] = from_clips
+    out["from_time"] = np.asarray(from_times, dtype=np.float32)
+    out["to_clip"] = np.asarray(to_clips, dtype=np.uint32)
+    out["to_time"] = np.asarray(to_times, dtype=np.float32)
     return out
 
 
@@ -412,6 +429,18 @@ class Context:
                                                               _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
                                                               _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
+    def decompress_tracks_blend(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, weight: float = 0.5,
+                                d_weights=None, d_parent_indices=None, kind: int = 0, d_skeleton_offsets=None, d_out_flags=None,
+                                stream=None) -> None:
+        """num_requests blend pairs (make_blend_requests): pose r = rtm::qvv_lerp(decode(from), decode(to), w), w = d_weights[r] (float32,
+        None: `weight` for every pair), used as given. With d_parent_indices the blended pose leaves in object space as `kind` rows
+        (OBJECT_*), the skeleton of the from clip c at d_parent_indices + d_skeleton_offsets[c]; without, in options.output_layout.
+        d_out_flags: optional uint32 ERROR_FLAG_* of the walk."""
+        self._check(_lib().aclb200_decompress_tracks_blend(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                           C.byref(options), weight, _device_ptr(d_weights), _device_ptr(d_parent_indices),
+                                                           _device_ptr(d_skeleton_offsets), kind, _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                           _stream_ptr(stream)))
+
     def decompress_track(self, clipset: ClipSet, d_requests, d_track_indices, num_requests: int, options: Options, d_out, stream=None) -> None:
         self._check(_lib().aclb200_decompress_track(self._handle, clipset._handle, _device_ptr(d_requests), _device_ptr(d_track_indices),
                                                     num_requests, C.byref(options), _device_ptr(d_out), _stream_ptr(stream)))
@@ -473,6 +502,13 @@ class Context:
         self._check(_lib().aclb200_apply_additive_to_base(self._handle, _device_ptr(d_base_poses), _device_ptr(d_additive_poses), _device_ptr(d_out),
                                                           num_poses, num_tracks, pose_stride_bytes, additive_format, _device_ptr(d_out_flags),
                                                           _stream_ptr(stream)))
+
+    def blend_poses(self, d_from_poses, d_to_poses, d_out, num_poses: int, num_tracks: int, weight: float = 0.5, d_weights=None,
+                    pose_stride_bytes: int = 0, stream=None) -> None:
+        """rtm::qvv_lerp(from, to, w) on every bone of num_poses QVV48 poses, w = d_weights[p] (float32) or `weight`; d_out may be
+        either input."""
+        self._check(_lib().aclb200_blend_poses(self._handle, _device_ptr(d_from_poses), _device_ptr(d_to_poses), _device_ptr(d_out), num_poses,
+                                               num_tracks, pose_stride_bytes, weight, _device_ptr(d_weights), _stream_ptr(stream)))
 
     # ---- host buffers in, host buffers out (the call the C++ header shim uses) ----
     def decompress_tracks_host(self, clipset: ClipSet, requests: np.ndarray, options: Options, out: np.ndarray) -> np.ndarray:

@@ -1,6 +1,7 @@
 // acl_b200/csrc/api.cpp -- the extern "C" surface declared in include/aclb200.h.
 #include "context.h"
 
+#include <cstddef>
 #include <cstring>
 #include <functional>
 #include <new>
@@ -19,7 +20,7 @@ namespace aclb200
 
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			bool object_space = false, bool additive_pairs = false)
+			bool object_space = false, uint32_t pairs = k_pairs_none)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -106,10 +107,12 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: an object transform needs every sub-track of its parents (no skip masks, no `skipped` default mode)");
 			if (object_space && options->output_layout != ACLB200_LAYOUT_QVV48)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: the output layout must be QVV48");
-			if (additive_pairs && (any_skipped || any_masked))
+			if (pairs == k_pairs_additive && (any_skipped || any_masked))
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: apply_additive_to_base needs every sub-track of both poses (no skip masks, no `skipped` default mode)");
+			if (pairs == k_pairs_blend && (any_skipped || any_masked))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: qvv_lerp needs every sub-track of both poses (no skip masks, no `skipped` default mode)");
 			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database,
-				object_space || additive_pairs, additive_pairs);
+				object_space || pairs != k_pairs_none, pairs != k_pairs_none);
 			return ACLB200_OK;
 		}
 
@@ -128,7 +131,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.7 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.8 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -374,7 +377,7 @@ extern "C"
 		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
 		DecodeParams params;
 		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, d_out,
-			true, false, params, false, true);
+			true, false, params, false, k_pairs_additive);
 		if (status != ACLB200_OK)
 			return status;
 		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
@@ -433,6 +436,68 @@ extern "C"
 		return finish_launch(context, launch_apply_additive(static_cast<const uint8_t*>(d_base_poses), static_cast<const uint8_t*>(d_additive_poses),
 			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, additive_format, d_out_flags, context->num_sms, cuda_stream),
 			"apply_additive_to_base");
+	}
+
+	aclb200_status aclb200_decompress_tracks_blend(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		float weight, const float* d_weights,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		if (num_requests > 0x7FFFFFFFu)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: more than 2^31 - 1 pairs");
+		// pair r is the two requests 2r (from) and 2r + 1 (to) of the plain decode, the layout of aclb200_additive_request
+		static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
+			"a blend request is two requests back to back");
+		DecodeParams params;
+		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, d_out,
+			true, false, params, false, k_pairs_blend);
+		if (status != ACLB200_OK)
+			return status;
+		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: unknown object_kind");
+		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: object space output needs the QVV48 layout");
+		// plan_launch kept both poses of a pair in shared memory and gave up key frame staging first: what is left must fit one block
+		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_blend: the two poses of a pair do not fit in a block's shared memory");
+		if (num_requests == 0)
+			return ACLB200_OK;
+		params.parent_indices = d_parent_indices;
+		params.skeleton_offsets = d_skeleton_offsets;
+		params.object_flags = d_out_flags;
+		params.object_kind = object_kind;
+		params.blend_weight = weight;
+		params.blend_weights = d_weights;
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		if (d_out_flags != nullptr)
+		{
+			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
+			if (cleared != cudaSuccess)
+				return check_cuda(context, cleared, "decompress_tracks_blend");
+		}
+		return finish_launch(context, launch_transform_decompress_tracks_blend(params, params.db_tiers != nullptr, cuda_stream),
+			"decompress_tracks_blend");
+	}
+
+	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,
+		uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, float weight, const float* d_weights, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		if (num_poses == 0 || num_tracks == 0)
+			return ACLB200_OK;
+		if (d_from_poses == nullptr || d_to_poses == nullptr || d_out == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "blend_poses: null pose pointer");
+		const uint64_t stride = pose_stride_bytes != 0 ? pose_stride_bytes : uint64_t(num_tracks) * 48;
+		if (stride < uint64_t(num_tracks) * 48 || (stride % 16) != 0
+			|| ((reinterpret_cast<uintptr_t>(d_from_poses) | reinterpret_cast<uintptr_t>(d_to_poses) | reinterpret_cast<uintptr_t>(d_out)) % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "blend_poses: poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		cudaSetDevice(context->device);
+		return finish_launch(context, launch_blend_poses(static_cast<const uint8_t*>(d_from_poses), static_cast<const uint8_t*>(d_to_poses),
+			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, weight, d_weights, context->num_sms, static_cast<cudaStream_t>(stream)),
+			"blend_poses");
 	}
 
 	aclb200_status aclb200_decompress_track(aclb200_context* context, const aclb200_clipset* clipset,

@@ -183,12 +183,18 @@ namespace aclb200
 		// parent_indices == nullptr there keeps the combined poses in local space
 		const uint8_t* clip_additive_formats;		// [num_clips] acl::additive_clip_format8 per additive clip (above 3: none), or nullptr
 		uint32_t additive_format;					// the format when clip_additive_formats == nullptr
+		// the blend decode (aclb200_decompress_tracks_blend): requests 2r / 2r + 1 are the from / to halves of pair r, output r
+		const float* blend_weights;					// [pairs] the weight of each pair, or nullptr
+		float blend_weight;							// the weight when blend_weights == nullptr
 	};
 
+	// the paired decodes of transform_decompress_tracks_kernel: pair r is requests 2r and 2r + 1, combined into output r
+	enum : uint32_t { k_pairs_none = 0, k_pairs_additive = 1, k_pairs_blend = 2 };
+
 	// kernels.cu
-	// additive_pairs: the additive decode, planned in whole pairs with both poses of a pair in shared memory
+	// pairs: a paired decode (additive or blend), planned in whole pairs with both poses of a pair in shared memory
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false,
-		bool force_output_staging = false, bool additive_pairs = false);
+		bool force_output_staging = false, bool pairs = false);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);
 	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
 	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
@@ -198,6 +204,9 @@ namespace aclb200
 	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream);
 	cudaError_t launch_apply_additive(const uint8_t* base_poses, const uint8_t* additive_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_tracks_blend(const DecodeParams& params, bool database, cudaStream_t stream);
+	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
+		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);
 	cudaError_t launch_transform_debug_unpack(const DecodeParams& params, uint32_t* d_out, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);

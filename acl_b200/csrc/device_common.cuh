@@ -217,7 +217,7 @@ namespace aclb200
 
 		// seek_v0 for transform clips, decompression.transform.h:206-563. DB == false: no database bound (a clip bound to one decodes
 		// from its resident key frames, as a context initialised without the database does). DB == true: the tier branches with the
-		// clip set's bound database (RS = ReqStateDB). PAIRED: requests 2r and 2r + 1 are the two halves of additive pair r, which share the
+		// clip set's bound database (RS = ReqStateDB). PAIRED: requests 2r and 2r + 1 are the two halves of pair r (additive or blend), sharing the
 		// per request policies of pair r.
 		template<bool DB = false, class RS = ReqState, bool PAIRED = false>
 		__device__ __forceinline__ void seek_transform(const DecodeParams& p, uint32_t request_index, RS& rs)

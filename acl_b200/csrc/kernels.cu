@@ -44,14 +44,17 @@ namespace aclb200
 		//             what the caller's buffer holds, or when a pose does not fit in shared memory)
 		// DB        : the clip set's bound database has chunks streamed in: key frames may come from its tier buffers
 		// OBJECT    : the staged poses are taken to object space before they leave (aclb200_decompress_tracks_object_space; OUT_STAGED, QVV48)
-		// ADDITIVE  : requests 2r and 2r + 1 are the base and the additive half of pair r (aclb200_decompress_tracks_additive; OUT_STAGED,
-		//             whole pairs per block). The additive half takes the track_writer defaults; phase 4c combines the two rows into row 2r,
-		//             which is taken to object space when parents are given (p.parent_indices, a run-time branch) and leaves as output r.
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false, bool OBJECT = false, bool ADDITIVE = false>
+		// PAIR      : k_pairs_additive or k_pairs_blend: requests 2r and 2r + 1 are the two halves of pair r (OUT_STAGED, whole pairs per
+		//             block); phase 4c combines the two rows into row 2r, which is taken to object space when parents are given
+		//             (p.parent_indices, a run-time branch) and leaves as output r.
+		//             additive (aclb200_decompress_tracks_additive): base and additive half; the additive half takes the track_writer defaults.
+		//             blend (aclb200_decompress_tracks_blend): from and to half, both full poses; row 2r becomes rtm::qvv_lerp(from, to, weight).
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false, bool OBJECT = false, uint32_t PAIR = k_pairs_none>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
-			static_assert(!ADDITIVE || (OUT_STAGED && !OBJECT), "the additive decode combines poses assembled in shared memory");
+			constexpr bool PAIRED = PAIR != k_pairs_none;
+			static_assert(!PAIRED || (OUT_STAGED && !OBJECT), "the paired decodes combine poses assembled in shared memory");
 			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
 			// dynamic shared memory: RS[requests_per_block] | key frame windows | pose staging
 			extern __shared__ __align__(16) uint8_t s_dynamic[];
@@ -75,7 +78,7 @@ namespace aclb200
 			if (threadIdx.x < num_requests)
 			{
 				RS rs;
-				seek_transform<DB, RS, ADDITIVE>(p, first_request + threadIdx.x, rs);
+				seek_transform<DB, RS, PAIRED>(p, first_request + threadIdx.x, rs);
 				rs.out = p.out + uint64_t(first_request + threadIdx.x) * p.pose_stride;
 				if (STAGED)
 				{
@@ -114,7 +117,8 @@ namespace aclb200
 						continue;
 					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
 					uint8_t* pose = OUT_STAGED ? s_out + size_t(local_request) * p.smem_pose_bytes : rs.out;
-					constant_sub_tracks<NORM, false>(p, rs, bone, desc, pose + size_t(bone) * p.bone_stride, ADDITIVE && (local_request & 1u) != 0);
+					constant_sub_tracks<NORM, false>(p, rs, bone, desc, pose + size_t(bone) * p.bone_stride,
+						PAIR == k_pairs_additive && (local_request & 1u) != 0);
 				}
 			}
 
@@ -170,7 +174,7 @@ namespace aclb200
 
 			// ---- phase 4c: one thread per (pair, bone) applies the additive row (request 2r + 1) to the base row (request 2r), in place;
 			// a pair whose halves differ in bone count (or name an invalid clip) is left alone and never stored ----
-			if constexpr (ADDITIVE)
+			if constexpr (PAIR == k_pairs_additive)
 			{
 				__syncthreads();
 				uint32_t flags = 0;
@@ -197,20 +201,40 @@ namespace aclb200
 					atomicOr(p.object_flags, flags);
 			}
 
-			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (ADDITIVE: the
+			// ---- phase 4c, blend: one thread per (pair, bone) lerps the from row (request 2r) towards the to row (request 2r + 1), in place,
+			// with the pair's weight; pairs whose halves differ in bone count are left alone as above ----
+			if constexpr (PAIR == k_pairs_blend)
+			{
+				__syncthreads();
+				const uint32_t first_pair = first_request >> 1;
+				const uint32_t num_slots = (num_requests >> 1) * p.max_tracks;
+				for (uint32_t slot = threadIdx.x; slot < num_slots; slot += k_threads_per_block)
+				{
+					const uint32_t pair = fast_div(slot, p.magic_tracks);
+					const uint32_t bone = slot - pair * p.max_tracks;
+					const uint32_t from_tracks = s_req[2 * pair].num_tracks;
+					if (bone >= from_tracks || s_req[2 * pair + 1].num_tracks != from_tracks)
+						continue;
+					const float weight = p.blend_weights != nullptr ? __ldg(p.blend_weights + first_pair + pair) : p.blend_weight;
+					uint8_t* row = s_out + size_t(2 * pair) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
+					obj::blend_row(row, row, row + p.smem_pose_bytes, weight, p.layout == ACLB200_LAYOUT_QVV40);
+				}
+			}
+
+			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (PAIRED: the
 			// combined row of each pair, when parents are given) ----
-			if constexpr (OBJECT || ADDITIVE)
+			if constexpr (OBJECT || PAIRED)
 			{
 				static_assert(OUT_STAGED, "the object space walk runs on poses assembled in shared memory");
-				if (!ADDITIVE || p.parent_indices != nullptr)
+				if (!PAIRED || p.parent_indices != nullptr)
 				{
 					__syncthreads();
 					uint32_t flags = 0;
-					constexpr uint32_t step = ADDITIVE ? 2u : 1u;
+					constexpr uint32_t step = PAIRED ? 2u : 1u;
 					for (uint32_t local_request = (threadIdx.x >> 5) * step; local_request < num_requests; local_request += (k_threads_per_block / 32) * step)
 					{
 						const RS& rs = s_req[local_request];
-						if (rs.num_tracks == 0 || (ADDITIVE && s_req[local_request + 1].num_tracks != rs.num_tracks))
+						if (rs.num_tracks == 0 || (PAIRED && s_req[local_request + 1].num_tracks != rs.num_tracks))
 							continue;
 						const uint32_t* parents = p.parent_indices + (p.skeleton_offsets != nullptr ? __ldg(p.skeleton_offsets + rs.clip) : 0u);
 						flags |= obj::pose_rows_to_object_space(s_out + size_t(local_request) * p.smem_pose_bytes, rs.num_tracks, parents,
@@ -222,22 +246,22 @@ namespace aclb200
 				}
 			}
 
-			// ---- phase 5: the assembled poses leave shared memory as full, coalesced 16 byte (or 8 byte) stores (ADDITIVE: row 2r of each
+			// ---- phase 5: the assembled poses leave shared memory as full, coalesced 16 byte (or 8 byte) stores (PAIRED: row 2r of each
 			// pair whose halves match, as output r) ----
 			if (OUT_STAGED)
 			{
 				__syncthreads();
 				const uint32_t chunks_per_pose = p.smem_pose_bytes >> 4;
-				const uint32_t num_poses = ADDITIVE ? num_requests >> 1 : num_requests;
-				const uint32_t first_pose = ADDITIVE ? first_request >> 1 : first_request;
+				const uint32_t num_poses = PAIRED ? num_requests >> 1 : num_requests;
+				const uint32_t first_pose = PAIRED ? first_request >> 1 : first_request;
 				const uint32_t num_chunks = num_poses * chunks_per_pose;
 				for (uint32_t slot = threadIdx.x; slot < num_chunks; slot += k_threads_per_block)
 				{
 					const uint32_t local_pose = fast_div(slot, p.magic_chunks);
-					const uint32_t local_request = ADDITIVE ? local_pose * 2 : local_pose;
+					const uint32_t local_request = PAIRED ? local_pose * 2 : local_pose;
 					const uint32_t byte = (slot - local_pose * chunks_per_pose) << 4;
 					uint32_t row_bytes = s_req[local_request].num_tracks * p.bone_stride;
-					if (ADDITIVE && s_req[local_request + 1].num_tracks != s_req[local_request].num_tracks)
+					if (PAIRED && s_req[local_request + 1].num_tracks != s_req[local_request].num_tracks)
 						row_bytes = 0;
 					if (byte >= row_bytes)
 						continue;
@@ -791,15 +815,15 @@ namespace aclb200
 			return cudaGetLastError();
 		}
 
-		// The additive decode: params.num_requests = 2 x pairs, params.requests_per_block even (plan_launch(..., additive_pairs = true))
-		template<int NORM, bool PER_TRACK, bool DB>
-		cudaError_t launch_tracks_additive(const DecodeParams& params, cudaStream_t stream)
+		// The paired decodes: params.num_requests = 2 x pairs, params.requests_per_block even (plan_launch(..., pairs = true))
+		template<int NORM, bool PER_TRACK, bool DB, uint32_t PAIR>
+		cudaError_t launch_tracks_pairs(const DecodeParams& params, cudaStream_t stream)
 		{
 			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
 			if (params.stage_bytes != 0)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB, false, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB, false, PAIR><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			else
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB, false, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB, false, PAIR><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
 			return cudaGetLastError();
 		}
 
@@ -822,6 +846,21 @@ namespace aclb200
 				atomicOr(out_flags, flags);
 		}
 
+		// aclb200_blend_poses: one thread per (pose, bone) of QVV48 rows; out may be either input (a thread reads its two rows before it
+		// writes its own)
+		__global__ void __launch_bounds__(256)
+		blend_poses_kernel(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
+			uint64_t pose_stride, float weight, const float* weights)
+		{
+			const uint64_t num_items = num_poses * num_tracks;
+			for (uint64_t item = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; item < num_items; item += uint64_t(gridDim.x) * blockDim.x)
+			{
+				const uint64_t pose = item / num_tracks;
+				const uint64_t offset = pose * pose_stride + (item - pose * num_tracks) * 48;
+				obj::blend_row(out + offset, from_poses + offset, to_poses + offset, weights != nullptr ? __ldg(weights + pose) : weight, false);
+			}
+		}
+
 		template<int NORM, bool PER_TRACK, bool DB = false>
 		cudaError_t launch_track(const DecodeParams& params, cudaStream_t stream)
 		{
@@ -830,18 +869,18 @@ namespace aclb200
 			return cudaGetLastError();
 		}
 
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, bool OBJECT = false, bool ADDITIVE = false>
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, bool OBJECT = false, uint32_t PAIR = k_pairs_none>
 		cudaError_t set_smem_attribute_one(int optin_limit, int& min_available)
 		{
 			// the opt-in limit covers static + dynamic shared memory
 			cudaFuncAttributes attributes;
-			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, ADDITIVE>);
+			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, PAIR>);
 			if (error != cudaSuccess)
 				return error;
 			const int available = optin_limit - int(attributes.sharedSizeBytes);
 			if (available < min_available)
 				min_available = available;
-			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, ADDITIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
+			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
 		}
 
 		template<int NORM, bool PER_TRACK>
@@ -862,10 +901,14 @@ namespace aclb200
 					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, true>(optin_limit, min_available);
 				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, true>(optin_limit, min_available)
 					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, true>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, false, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, false, true>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, false, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, false, true>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, false, k_pairs_additive>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, false, k_pairs_additive>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, false, k_pairs_additive>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, false, k_pairs_additive>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, false, k_pairs_blend>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, false, k_pairs_blend>(optin_limit, min_available);
+				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, false, k_pairs_blend>(optin_limit, min_available)
+					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, false, k_pairs_blend>(optin_limit, min_available);
 			}
 			return error;
 		}
@@ -892,9 +935,9 @@ namespace aclb200
 	// requests_per_block, the division magics and the shared memory carve-up of a launch
 	// force_output_staging: the object space decode needs every pose in shared memory, so a pose that does not fit gives up key frame
 	// staging instead (params.smem_bytes then tells the caller whether one request fits at all)
-	// additive_pairs: requests_per_block stays even, so that the two halves of a pair always share a block
+	// pairs: requests_per_block stays even, so that the two halves of a pair always share a block
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
-		bool force_output_staging, bool additive_pairs)
+		bool force_output_staging, bool pairs)
 	{
 		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
@@ -909,8 +952,8 @@ namespace aclb200
 		uint32_t requests_per_block = k_target_items_per_block / max_tracks;
 		if (requests_per_block < 1) requests_per_block = 1;
 		if (requests_per_block > k_max_requests_per_block) requests_per_block = k_max_requests_per_block;
-		const uint32_t step = additive_pairs ? 2u : 1u;
-		if (additive_pairs)
+		const uint32_t step = pairs ? 2u : 1u;
+		if (pairs)
 			requests_per_block = requests_per_block < 2 ? 2u : (requests_per_block & ~1u);
 
 		auto bytes_needed = [&](uint32_t requests) { return requests * (state_bytes + 2 * stage_bytes + pose_bytes); };
@@ -999,22 +1042,33 @@ namespace aclb200
 		}
 	}
 
-	// The additive decode: both math modes run the exact kernels, as the object space decode does
-	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream)
+	// The paired decodes: both math modes run the exact kernels, as the object space decode does
+	template<uint32_t PAIR>
+	cudaError_t launch_transform_decompress_tracks_pairs(const DecodeParams& params, bool database, cudaStream_t stream)
 	{
 		const bool per_track = params.per_track_rounding != 0;
 		switch (params.normalization)
 		{
 		case ACLB200_NORMALIZE_NEVER:
-			return database ? (per_track ? launch_tracks_additive<0, true, true>(params, stream) : launch_tracks_additive<0, false, true>(params, stream))
-				: (per_track ? launch_tracks_additive<0, true, false>(params, stream) : launch_tracks_additive<0, false, false>(params, stream));
+			return database ? (per_track ? launch_tracks_pairs<0, true, true, PAIR>(params, stream) : launch_tracks_pairs<0, false, true, PAIR>(params, stream))
+				: (per_track ? launch_tracks_pairs<0, true, false, PAIR>(params, stream) : launch_tracks_pairs<0, false, false, PAIR>(params, stream));
 		case ACLB200_NORMALIZE_LERP_ONLY:
-			return database ? (per_track ? launch_tracks_additive<1, true, true>(params, stream) : launch_tracks_additive<1, false, true>(params, stream))
-				: (per_track ? launch_tracks_additive<1, true, false>(params, stream) : launch_tracks_additive<1, false, false>(params, stream));
+			return database ? (per_track ? launch_tracks_pairs<1, true, true, PAIR>(params, stream) : launch_tracks_pairs<1, false, true, PAIR>(params, stream))
+				: (per_track ? launch_tracks_pairs<1, true, false, PAIR>(params, stream) : launch_tracks_pairs<1, false, false, PAIR>(params, stream));
 		default:
-			return database ? (per_track ? launch_tracks_additive<2, true, true>(params, stream) : launch_tracks_additive<2, false, true>(params, stream))
-				: (per_track ? launch_tracks_additive<2, true, false>(params, stream) : launch_tracks_additive<2, false, false>(params, stream));
+			return database ? (per_track ? launch_tracks_pairs<2, true, true, PAIR>(params, stream) : launch_tracks_pairs<2, false, true, PAIR>(params, stream))
+				: (per_track ? launch_tracks_pairs<2, true, false, PAIR>(params, stream) : launch_tracks_pairs<2, false, false, PAIR>(params, stream));
 		}
+	}
+
+	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream)
+	{
+		return launch_transform_decompress_tracks_pairs<k_pairs_additive>(params, database, stream);
+	}
+
+	cudaError_t launch_transform_decompress_tracks_blend(const DecodeParams& params, bool database, cudaStream_t stream)
+	{
+		return launch_transform_decompress_tracks_pairs<k_pairs_blend>(params, database, stream);
 	}
 
 	cudaError_t launch_apply_additive(const uint8_t* base_poses, const uint8_t* additive_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
@@ -1023,6 +1077,15 @@ namespace aclb200
 		const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
 		const uint32_t blocks = uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
 		apply_additive_kernel<<<blocks, 256, 0, stream>>>(base_poses, additive_poses, out, num_poses, num_tracks, pose_stride, additive_format, flags);
+		return cudaGetLastError();
+	}
+
+	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
+		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream)
+	{
+		const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
+		const uint32_t blocks = uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
+		blend_poses_kernel<<<blocks, 256, 0, stream>>>(from_poses, to_poses, out, num_poses, num_tracks, pose_stride, weight, weights);
 		return cudaGetLastError();
 	}
 

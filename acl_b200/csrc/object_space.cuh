@@ -1,7 +1,8 @@
 // acl_b200/csrc/object_space.cuh -- the hierarchy walk shared by the error measurement (error_metric.cu: object_space_kernel) and the
 // object space decode (kernels.cu: transform_decompress_tracks_kernel<..., OBJECT = true>): the reference's qvv and 3x4 matrix operations
 // restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which the
-// error measurement, the additive decode (ADDITIVE = true) and aclb200_apply_additive_to_base share.
+// error measurement, the additive decode (PAIR = k_pairs_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which the
+// blend decode (PAIR = k_pairs_blend) and aclb200_blend_poses share.
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
@@ -577,6 +578,41 @@ namespace aclb200
 				}
 				store_pose_row(out_row, format == 0 ? additive : apply_additive_to_base_positive(fp, format, base, additive), qvv40);
 				return 0;
+			}
+
+			// rtm::vector_lerp, vector4f.h:2417-2421 with the SSE2 macros (macros.vector4.impl.h:93,152): (start - start * alpha) + end * alpha
+			__device__ __forceinline__ float lerp_lane(const Fp<float>& fp, float start, float end, float alpha)
+			{
+				return fp.add(fp.sub(start, fp.mul(start, alpha)), fp.mul(end, alpha));
+			}
+
+			// out_row = rtm::qvv_lerp(from_row, to_row, weight) (qvvf.h:439-445), rows as apply_additive_row's; out_row may be either input.
+			// quat_lerp is its SSE4.1 path (quatf.h:1006-1075): dot = _mm_dp_ps(start, end, 0xFF), which sums (x x' + y y') + (z z' + w w');
+			// the SIGN BIT of dot is xor-ed onto `end` (so dot == -0.0 flips it, unlike the scalar and NEON paths); (s - w s) + w (e ^ bias) per
+			// lane, then quat_normalize with the IEEE 1 / sqrt in place of rsqrtss + 2 Newton-Raphson steps. The weight is used as given: no
+			// clamp, below 0 and above 1 extrapolate.
+			__device__ __forceinline__ void blend_row(uint8_t* out_row, const uint8_t* from_row, const uint8_t* to_row, float weight, bool qvv40)
+			{
+				const Fp<float> fp{};
+				const Qvv<float> from = load_pose_row(from_row, qvv40);
+				const Qvv<float> to = load_pose_row(to_row, qvv40);
+				const Quat<float>& s = from.rotation;
+				const Quat<float>& e = to.rotation;
+				const float dot = fp.add(fp.add(fp.mul(s.x, e.x), fp.mul(s.y, e.y)), fp.add(fp.mul(s.z, e.z), fp.mul(s.w, e.w)));
+				const uint32_t bias = __float_as_uint(dot) & 0x80000000u;
+				const auto biased = [bias](float v) { return __uint_as_float(__float_as_uint(v) ^ bias); };
+				Quat<float> q;
+				q.x = fp.add(fp.sub(s.x, fp.mul(weight, s.x)), fp.mul(weight, biased(e.x)));
+				q.y = fp.add(fp.sub(s.y, fp.mul(weight, s.y)), fp.mul(weight, biased(e.y)));
+				q.z = fp.add(fp.sub(s.z, fp.mul(weight, s.z)), fp.mul(weight, biased(e.z)));
+				q.w = fp.add(fp.sub(s.w, fp.mul(weight, s.w)), fp.mul(weight, biased(e.w)));
+				Qvv<float> out;
+				out.rotation = quat_normalize(fp, q);
+				out.translation = Vec3<float>{ lerp_lane(fp, from.translation.x, to.translation.x, weight), lerp_lane(fp, from.translation.y, to.translation.y, weight),
+					lerp_lane(fp, from.translation.z, to.translation.z, weight) };
+				out.scale = Vec3<float>{ lerp_lane(fp, from.scale.x, to.scale.x, weight), lerp_lane(fp, from.scale.y, to.scale.y, weight),
+					lerp_lane(fp, from.scale.z, to.scale.z, weight) };
+				store_pose_row(out_row, out, qvv40);
 			}
 		}
 	}

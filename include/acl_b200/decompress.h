@@ -429,6 +429,23 @@ namespace acl_b200
 			m_device->check(aclb200_apply_additive_to_base(m_device->get(), d_base_poses, d_additive_poses, d_out, num_poses, num_tracks, pose_stride_bytes,
 				additive_format, d_out_flags, stream), "aclb200_apply_additive_to_base");
 		}
+		// decompress from + decompress to + rtm::qvv_lerp(from, to, w) per bone, in one launch (aclb200_decompress_tracks_blend); w =
+		// d_weights[r] (nullptr: weight). With parents the blended pose leaves in object space as object_kind rows (the from clip's
+		// skeleton), else as local rows in options.output_layout.
+		void decompress_tracks_blend(const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			float weight, const float* d_weights, void* d_out, const uint32_t* d_parent_indices = nullptr, const uint32_t* d_skeleton_offsets = nullptr,
+			uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_blend(m_device->get(), m_clipset, d_requests, num_requests, &options, weight, d_weights,
+				d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_blend");
+		}
+		// rtm::qvv_lerp(from, to, w) over num_poses QVV48 poses already on the device (aclb200_blend_poses); d_out may be either input
+		void blend_poses(const void* d_from_poses, const void* d_to_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, float weight,
+			const float* d_weights = nullptr, uint64_t pose_stride_bytes = 0, void* stream = nullptr)
+		{
+			m_device->check(aclb200_blend_poses(m_device->get(), d_from_poses, d_to_poses, d_out, num_poses, num_tracks, pose_stride_bytes, weight,
+				d_weights, stream), "aclb200_blend_poses");
+		}
 		// host buffers in, host buffers out, synchronous
 		void decompress_tracks_host(const aclb200_request* requests, uint32_t num_requests, const aclb200_options& options, void* out, size_t out_bytes)
 		{

@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 7
+#define ACLB200_VERSION_MINOR 8
 
 typedef enum aclb200_status
 {
@@ -458,6 +458,50 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_additive(aclb200_context* c
 ACLB200_API aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
 	void* d_out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, uint32_t additive_format,
 	uint32_t* d_out_flags, void* stream);
+
+/* One blended pose: two clips of the same clip set, each at its own sample time (a crossfade, or a blend of walk and run) */
+typedef struct aclb200_blend_request
+{
+	aclb200_request from;			/* weight 0 gives this pose */
+	aclb200_request to;				/* weight 1 gives this pose (or its hemisphere-flipped rotation) */
+} aclb200_blend_request;
+
+/* decompress from + decompress to + rtm::qvv_lerp(from, to, w) (rtm/qvvf.h:439-445) per bone, in one kernel: neither pose leaves shared
+ * memory. For pair r:
+ *   both poses     what aclb200_decompress_tracks computes for requests[r].from and requests[r].to with `options` (rounding, looping, per
+ *                  request policies -- d_request_policies[r] applies to both halves --, per track rounding, normalisation, default modes and
+ *                  bind pose, a bound database's streamed tiers). Neither half takes the track_writer defaults: both are full poses.
+ *   w              d_weights[r] (device float[num_requests]) when d_weights is not NULL, else `weight`; used as given, no clamp: below 0 and
+ *                  above 1 extrapolate, as rtm does
+ *   blend          rtm::quat_lerp's SSE4.1 path: dot = (x x' + y y') + (z z' + w w'); `to`'s rotation is negated when the SIGN BIT of dot is
+ *                  set (dot == -0.0 included); q = (s - w s) + w to per lane, then quat_normalize with an IEEE 1 / sqrt (the reference's
+ *                  rsqrtss + 2 Newton-Raphson steps is CPU specific: rotations agree within 1e-6). Translations and scales are
+ *                  rtm::vector_lerp: (s - s w) + e w, bit-identical to the reference. The translation and scale w lanes are written as 0.
+ *   d_out          d_parent_indices == NULL: the blended local pose in options->output_layout at d_out + r * options->pose_stride_bytes
+ *                  (0 = max_tracks * bone size). d_parent_indices given: the blended local pose goes through the hierarchy walk of
+ *                  aclb200_decompress_tracks_object_space with the skeleton d_parent_indices + d_skeleton_offsets[requests[r].from.clip]
+ *                  (d_skeleton_offsets NULL: 0) and leaves as object_kind rows (QVV48 only): blend in local space, then to object space.
+ *                  A pair with an invalid clip index on either side, or with clips of different track counts, writes nothing; no byte
+ *                  past a clip's num_tracks bones is written.
+ *   d_out_flags    device uint32, optional: cleared, then the walk's ACLB200_ERROR_FLAG_NEGATIVE_SCALE and ACLB200_ERROR_FLAG_INVALID_SKELETON
+ *                  OR-ed in (the blend itself raises none)
+ * Every operation is IEEE and unfused; ACLB200_MATH_FAST is accepted and runs the exact decode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, writing nothing: skip masks, a `skipped` default mode, a scalar clip set, an output that breaks
+ * the alignment rules of aclb200_decompress_tracks, and with parents an unknown object_kind or QVV40.
+ * ACLB200_ERR_UNSUPPORTED when the two poses of a pair do not fit in one block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_blend(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	float weight, const float* d_weights,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* rtm::qvv_lerp(from, to, w) as aclb200_decompress_tracks_blend computes it, on every bone of num_poses poses of rtm::qvvf rows (48 byte
+ * bones, 16 byte aligned; pose p of each buffer at p * pose_stride_bytes, 0 = num_tracks * 48), w = d_weights[p] (device float[num_poses])
+ * or `weight` when d_weights is NULL: for poses already on the device, such as a chain of blends (a 2D blend space is lerps of lerps) or a
+ * decoded pose and a pose from elsewhere. d_out may be either input. The translation and scale w lanes are written as 0.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT: NULL pointers, misaligned rows. */
+ACLB200_API aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,
+	uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, float weight, const float* d_weights, void* stream);
 
 /* Parity / debugging hooks (integer stages of the decode, bit-exact against the reference):
  *  - aclb200_debug_seek: the state seek_v0 computes, one aclb200_seek_state per request (device output).

@@ -1,7 +1,8 @@
 """Small workload for compute-sanitizer (tools/sanitize.sh): every kernel of the library once or twice, checked against the oracle --
 chained playback through the pipeline kernel (groups, tail crossing, base row reuse), ragged random requests, per track rounding,
 skipped defaults (plain kernels), decompress_track, the object space decode (both kinds, a skeleton per clip), the additive decode (local and
-object space, per clip formats) and aclb200_apply_additive_to_base, the chained scalar kernel."""
+object space, per clip formats) and aclb200_apply_additive_to_base, the blend decode (local and object space, a weight per pair) and
+aclb200_blend_poses, the chained scalar kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -90,6 +91,28 @@ for parents in (None, d_parents):
             want = port.local_to_object_space(want, trees[c], port.NORMALIZE_IEEE)
         bad += not clips.bit_equal(got[i, :counts[c]][:, L], want[:, L])
 ctx.apply_additive_to_base(out, out, out, len(pairs), cs.max_tracks, ab.ADDITIVE_ADDITIVE0)
+torch.cuda.synchronize()
+# blend decode: the PAIR = blend instances (pairs of clips with equal bone counts, a weight per pair, local then object space) and the
+# standalone blend_poses_kernel, in place
+from oracle import blend
+blend_pairs = ab.make_blend_requests(pair_clip, pair_time[:, 0], pair_clip, pair_time[:, 1])
+d_blend_pairs = torch.from_numpy(blend_pairs.view(np.uint8)).cuda()
+blend_weights = rng.uniform(-0.25, 1.25, len(blend_pairs)).astype(np.float32)
+d_blend_weights = torch.from_numpy(blend_weights).cuda()
+for parents in (None, d_parents):
+    out = torch.zeros((len(blend_pairs), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+    ctx.decompress_tracks_blend(cs, d_blend_pairs, len(blend_pairs), ab.Options(), out, d_weights=d_blend_weights, d_parent_indices=parents,
+                                d_skeleton_offsets=d_offsets)
+    torch.cuda.synchronize()
+    got = out.cpu().numpy()
+    for i in range(0, len(blend_pairs), 5):
+        c = pair_clip[i]
+        want = blend.port_qvv_lerp(port.transform_decompress_tracks(blobs[c], settings, float(pair_time[i, 0])),
+                                   port.transform_decompress_tracks(blobs[c], settings, float(pair_time[i, 1])), float(blend_weights[i]))
+        if parents is not None:
+            want = port.local_to_object_space(want, trees[c], port.NORMALIZE_IEEE)
+        bad += not clips.bit_equal(got[i, :counts[c]][:, L], want[:, L])
+ctx.blend_poses(out, out, out, len(blend_pairs), cs.max_tracks, d_weights=d_blend_weights)
 torch.cuda.synchronize()
 # scalar clips
 for name in ("float1", "float3", "vector4", "float1_c4_small"):
