@@ -18,9 +18,20 @@ namespace aclb200
 			return track_type <= 3 ? track_type + 1 : 4;
 		}
 
+		// `skipped` default sub-tracks and skipped sub-tracks (track_writer::skip_*) keep what the caller's buffer holds
+		bool keeps_caller_bytes(const aclb200_options& options)
+		{
+			return options.default_rotation_mode == ACLB200_DEFAULT_SKIPPED || options.default_translation_mode == ACLB200_DEFAULT_SKIPPED
+				|| options.default_scale_mode == ACLB200_DEFAULT_SKIPPED || (options.skip_mask & 7u) != 0 || options.d_skip_track_mask != nullptr;
+		}
+
+		// the C entry point of each compose mode, for messages
+		const char* const k_compose_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_object_space", "decompress_tracks_additive",
+			"decompress_tracks_blend" };
+
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			bool object_space = false, uint32_t pairs = k_pairs_none)
+			uint32_t compose = k_compose_local)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -86,12 +97,9 @@ namespace aclb200
 			params.skip_tracks = is_transform ? options->d_skip_track_mask : nullptr;
 			params.request_policies = options->d_request_policies;
 			params.layout = options->output_layout;
-			// `skipped` default sub-tracks must keep what the caller's buffer holds: those launches store sub-tracks straight to
-			// global memory instead of assembling whole poses in shared memory
-			const bool any_skipped = options->default_rotation_mode == ACLB200_DEFAULT_SKIPPED || options->default_translation_mode == ACLB200_DEFAULT_SKIPPED
-				|| options->default_scale_mode == ACLB200_DEFAULT_SKIPPED;
-			// ... and so must skipped sub-tracks (track_writer::skip_*)
-			const bool any_masked = (options->skip_mask & 7u) != 0 || options->d_skip_track_mask != nullptr;
+			// launches that keep the caller's bytes store sub-tracks straight to global memory instead of assembling whole poses in
+			// shared memory
+			const bool keeps_bytes = keeps_caller_bytes(*options);
 			const bool tracks_launch = is_transform && !single_track;
 			// a bound database with chunks streamed in: the launch takes the database kernels (with nothing streamed in, the resident key
 			// frames give the reference's result, so every other launch runs the kernels it always did)
@@ -103,16 +111,11 @@ namespace aclb200
 				params.db_bulk[0] = clipset->database->d_bulk[0];
 				params.db_bulk[1] = clipset->database->d_bulk[1];
 			}
-			if (object_space && (any_skipped || any_masked))
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: an object transform needs every sub-track of its parents (no skip masks, no `skipped` default mode)");
-			if (object_space && options->output_layout != ACLB200_LAYOUT_QVV48)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: the output layout must be QVV48");
-			if (pairs == k_pairs_additive && (any_skipped || any_masked))
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: apply_additive_to_base needs every sub-track of both poses (no skip masks, no `skipped` default mode)");
-			if (pairs == k_pairs_blend && (any_skipped || any_masked))
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: qvv_lerp needs every sub-track of both poses (no skip masks, no `skipped` default mode)");
-			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !any_skipped && !any_masked, database,
-				object_space || pairs != k_pairs_none, pairs != k_pairs_none);
+			// an object transform needs every sub-track of its parents, apply_additive_to_base and qvv_lerp every sub-track of both poses
+			if (compose != k_compose_local && keeps_bytes)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(k_compose_entry[compose])
+					+ ": the composed poses need every decoded sub-track (no skip masks, no `skipped` default mode)");
+			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !keeps_bytes, database, compose);
 			return ACLB200_OK;
 		}
 
@@ -122,6 +125,60 @@ namespace aclb200
 				context->launch_count++;
 			return check_cuda(context, error, what);
 		}
+
+		// The composed decodes. Every refusal comes before the flags are cleared: a refused call writes nothing.
+		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, uint32_t compose, const uint32_t* d_parent_indices,
+			const uint32_t* d_skeleton_offsets, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream,
+			const std::function<void(DecodeParams&)>& set_pair_operands = nullptr)
+		{
+			const std::string entry = k_compose_entry[compose];
+			DecodeParams params;
+			const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, compose);
+			if (status != ACLB200_OK)
+				return status;
+			// object space output: always in the object space decode (its entry point requires parents), with parents in the paired ones
+			if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": unknown object_kind");
+			if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
+			// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
+			if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
+				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + (compose == k_compose_object ? ": one pose does not fit in a block's shared memory"
+					: ": the two poses of a pair do not fit in a block's shared memory"));
+			if (num_requests == 0)
+				return ACLB200_OK;
+			params.parent_indices = d_parent_indices;
+			params.skeleton_offsets = d_skeleton_offsets;
+			params.object_flags = d_out_flags;
+			params.object_kind = object_kind;
+			if (set_pair_operands)
+				set_pair_operands(params);
+			cudaSetDevice(context->device);
+			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+			const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, entry.c_str());
+			if (cleared != ACLB200_OK)
+				return cleared;
+			return finish_launch(context, launch_transform_decompress_tracks(params, compose, params.db_tiers != nullptr, cuda_stream), entry.c_str());
+		}
+	}
+
+	aclb200_status clear_out_flags(aclb200_context* context, uint32_t* d_out_flags, cudaStream_t stream, const char* what)
+	{
+		return d_out_flags != nullptr ? check_cuda(context, cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), stream), what) : ACLB200_OK;
+	}
+
+	aclb200_status check_qvvf_rows(aclb200_context* context, std::initializer_list<const void*> poses, uint32_t num_tracks, uint64_t& pose_stride,
+		const char* what)
+	{
+		if (pose_stride == 0)
+			pose_stride = uint64_t(num_tracks) * 48;
+		uintptr_t addresses = 0;
+		for (const void* pose : poses)
+			addresses |= reinterpret_cast<uintptr_t>(pose);
+		if (pose_stride < uint64_t(num_tracks) * 48 || (pose_stride % 16) != 0 || (addresses % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		return ACLB200_OK;
 	}
 }
 
@@ -298,15 +355,13 @@ extern "C"
 		if (params.db_tiers != nullptr)
 		{
 			launch.kernel = ACLB200_KERNEL_DATABASE;
-			return finish_launch(context, launch_transform_decompress_tracks_database(params, static_cast<cudaStream_t>(stream)), "decompress_tracks (database)");
+			return finish_launch(context, launch_transform_decompress_tracks(params, k_compose_local, true, static_cast<cudaStream_t>(stream)),
+				"decompress_tracks (database)");
 		}
 
 		// Main path: the persistent TMA pipeline (pipeline.cu). It assembles whole poses in shared memory, so launches that must
 		// leave `skipped` default sub-tracks untouched, or whose poses do not fit in shared memory, use the plain kernels instead.
-		const bool any_skipped = options->default_rotation_mode == ACLB200_DEFAULT_SKIPPED || options->default_translation_mode == ACLB200_DEFAULT_SKIPPED
-			|| options->default_scale_mode == ACLB200_DEFAULT_SKIPPED;
-		const bool any_masked = (options->skip_mask & 7u) != 0 || options->d_skip_track_mask != nullptr;
-		if (!any_skipped && !any_masked && clipset->max_key_frame_bytes != 0)
+		if (!keeps_caller_bytes(*options) && clipset->max_key_frame_bytes != 0)
 		{
 			DecodeParams pipeline_params = params;
 			if (plan_pipeline(pipeline_params, clipset->max_key_frame_bytes, context->max_dynamic_smem, context->num_sms))
@@ -328,7 +383,7 @@ extern "C"
 			}
 		}
 		launch.kernel = ACLB200_KERNEL_PLAIN;
-		return finish_launch(context, launch_transform_decompress_tracks(params, options->math_mode, static_cast<cudaStream_t>(stream)), "decompress_tracks");
+		return finish_launch(context, launch_transform_decompress_tracks(params, k_compose_local, false, static_cast<cudaStream_t>(stream)), "decompress_tracks");
 	}
 
 	aclb200_status aclb200_decompress_tracks_object_space(aclb200_context* context, const aclb200_clipset* clipset,
@@ -336,33 +391,10 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		DecodeParams params;
-		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, true);
-		if (status != ACLB200_OK)
-			return status;
-		if (object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: unknown object_kind");
 		if (d_parent_indices == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: null parent index pointer");
-		// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
-		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_object_space: one pose does not fit in a block's shared memory");
-		if (num_requests == 0)
-			return ACLB200_OK;
-		params.parent_indices = d_parent_indices;
-		params.skeleton_offsets = d_skeleton_offsets;
-		params.object_flags = d_out_flags;
-		params.object_kind = object_kind;
-		cudaSetDevice(context->device);
-		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		if (d_out_flags != nullptr)
-		{
-			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
-			if (cleared != cudaSuccess)
-				return check_cuda(context, cleared, "decompress_tracks_object_space");
-		}
-		return finish_launch(context, launch_transform_decompress_tracks_object_space(params, params.db_tiers != nullptr, cuda_stream),
-			"decompress_tracks_object_space");
+		return decompress_composed(context, clipset, d_requests, num_requests, options, k_compose_object, d_parent_indices, d_skeleton_offsets,
+			object_kind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
@@ -373,40 +405,16 @@ extern "C"
 	{
 		if (num_requests > 0x7FFFFFFFu)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: more than 2^31 - 1 pairs");
-		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
-		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
-		DecodeParams params;
-		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, d_out,
-			true, false, params, false, k_pairs_additive);
-		if (status != ACLB200_OK)
-			return status;
 		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: additive_format out of range");
-		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: unknown object_kind");
-		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: object space output needs the QVV48 layout");
-		// plan_launch kept both poses of a pair in shared memory and gave up key frame staging first: what is left must fit one block
-		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_additive: the two poses of a pair do not fit in a block's shared memory");
-		if (num_requests == 0)
-			return ACLB200_OK;
-		params.parent_indices = d_parent_indices;
-		params.skeleton_offsets = d_skeleton_offsets;
-		params.object_flags = d_out_flags;
-		params.object_kind = object_kind;
-		params.additive_format = additive_format;
-		params.clip_additive_formats = d_clip_additive_formats;
-		cudaSetDevice(context->device);
-		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		if (d_out_flags != nullptr)
-		{
-			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
-			if (cleared != cudaSuccess)
-				return check_cuda(context, cleared, "decompress_tracks_additive");
-		}
-		return finish_launch(context, launch_transform_decompress_tracks_additive(params, params.db_tiers != nullptr, cuda_stream),
-			"decompress_tracks_additive");
+		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
+		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_additive,
+			d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			{
+				params.additive_format = additive_format;
+				params.clip_additive_formats = d_clip_additive_formats;
+			});
 	}
 
 	aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
@@ -421,18 +429,15 @@ extern "C"
 			return ACLB200_OK;
 		if (d_base_poses == nullptr || d_additive_poses == nullptr || d_out == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: null pose pointer");
-		const uint64_t stride = pose_stride_bytes != 0 ? pose_stride_bytes : uint64_t(num_tracks) * 48;
-		if (stride < uint64_t(num_tracks) * 48 || (stride % 16) != 0
-			|| ((reinterpret_cast<uintptr_t>(d_base_poses) | reinterpret_cast<uintptr_t>(d_additive_poses) | reinterpret_cast<uintptr_t>(d_out)) % 16) != 0)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		uint64_t stride = pose_stride_bytes;
+		aclb200_status status = check_qvvf_rows(context, { d_base_poses, d_additive_poses, d_out }, num_tracks, stride, "apply_additive_to_base");
+		if (status != ACLB200_OK)
+			return status;
 		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		if (d_out_flags != nullptr)
-		{
-			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
-			if (cleared != cudaSuccess)
-				return check_cuda(context, cleared, "apply_additive_to_base");
-		}
+		status = clear_out_flags(context, d_out_flags, cuda_stream, "apply_additive_to_base");
+		if (status != ACLB200_OK)
+			return status;
 		return finish_launch(context, launch_apply_additive(static_cast<const uint8_t*>(d_base_poses), static_cast<const uint8_t*>(d_additive_poses),
 			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, additive_format, d_out_flags, context->num_sms, cuda_stream),
 			"apply_additive_to_base");
@@ -449,36 +454,12 @@ extern "C"
 		// pair r is the two requests 2r (from) and 2r + 1 (to) of the plain decode, the layout of aclb200_additive_request
 		static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
 			"a blend request is two requests back to back");
-		DecodeParams params;
-		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, d_out,
-			true, false, params, false, k_pairs_blend);
-		if (status != ACLB200_OK)
-			return status;
-		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: unknown object_kind");
-		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: object space output needs the QVV48 layout");
-		// plan_launch kept both poses of a pair in shared memory and gave up key frame staging first: what is left must fit one block
-		if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-			return set_error(context, ACLB200_ERR_UNSUPPORTED, "decompress_tracks_blend: the two poses of a pair do not fit in a block's shared memory");
-		if (num_requests == 0)
-			return ACLB200_OK;
-		params.parent_indices = d_parent_indices;
-		params.skeleton_offsets = d_skeleton_offsets;
-		params.object_flags = d_out_flags;
-		params.object_kind = object_kind;
-		params.blend_weight = weight;
-		params.blend_weights = d_weights;
-		cudaSetDevice(context->device);
-		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		if (d_out_flags != nullptr)
-		{
-			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
-			if (cleared != cudaSuccess)
-				return check_cuda(context, cleared, "decompress_tracks_blend");
-		}
-		return finish_launch(context, launch_transform_decompress_tracks_blend(params, params.db_tiers != nullptr, cuda_stream),
-			"decompress_tracks_blend");
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_blend,
+			d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			{
+				params.blend_weight = weight;
+				params.blend_weights = d_weights;
+			});
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,
@@ -490,10 +471,10 @@ extern "C"
 			return ACLB200_OK;
 		if (d_from_poses == nullptr || d_to_poses == nullptr || d_out == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "blend_poses: null pose pointer");
-		const uint64_t stride = pose_stride_bytes != 0 ? pose_stride_bytes : uint64_t(num_tracks) * 48;
-		if (stride < uint64_t(num_tracks) * 48 || (stride % 16) != 0
-			|| ((reinterpret_cast<uintptr_t>(d_from_poses) | reinterpret_cast<uintptr_t>(d_to_poses) | reinterpret_cast<uintptr_t>(d_out)) % 16) != 0)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "blend_poses: poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		uint64_t stride = pose_stride_bytes;
+		const aclb200_status status = check_qvvf_rows(context, { d_from_poses, d_to_poses, d_out }, num_tracks, stride, "blend_poses");
+		if (status != ACLB200_OK)
+			return status;
 		cudaSetDevice(context->device);
 		return finish_launch(context, launch_blend_poses(static_cast<const uint8_t*>(d_from_poses), static_cast<const uint8_t*>(d_to_poses),
 			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, weight, d_weights, context->num_sms, static_cast<cudaStream_t>(stream)),
@@ -512,9 +493,9 @@ extern "C"
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null track index pointer");
 		params.track_indices = d_track_indices;
 		cudaSetDevice(context->device);
-		if (params.db_tiers != nullptr)
-			return finish_launch(context, launch_transform_decompress_track_database(params, static_cast<cudaStream_t>(stream)), "decompress_track (database)");
-		return finish_launch(context, launch_transform_decompress_track(params, options->math_mode, static_cast<cudaStream_t>(stream)), "decompress_track");
+		const bool database = params.db_tiers != nullptr;
+		return finish_launch(context, launch_transform_decompress_track(params, database, static_cast<cudaStream_t>(stream)),
+			database ? "decompress_track (database)" : "decompress_track");
 	}
 
 	aclb200_status aclb200_scalar_decompress_tracks(aclb200_context* context, const aclb200_clipset* clipset,
@@ -594,9 +575,7 @@ extern "C"
 			return check_cuda(context, error, "decompress_tracks_host: streams");
 
 		// `skipped` default sub-tracks keep what the caller's buffer held: bring the buffer in first in that case
-		const bool keeps_input = is_transform && (options->default_rotation_mode == ACLB200_DEFAULT_SKIPPED
-			|| options->default_translation_mode == ACLB200_DEFAULT_SKIPPED || options->default_scale_mode == ACLB200_DEFAULT_SKIPPED
-			|| (options->skip_mask & 7u) != 0 || options->d_skip_track_mask != nullptr);
+		const bool keeps_input = is_transform && keeps_caller_bytes(*options);
 		// Rows no request writes (clips shorter than the widest one, requests naming a clip outside the set) read as zero. Clearing the
 		// scratch costs a pass over it, so it only happens when such rows can exist.
 		bool needs_clear = !keeps_input && (clipset->info.min_tracks != clipset->info.max_tracks || pose_stride != uint64_t(clipset->info.max_tracks) * bone_stride);

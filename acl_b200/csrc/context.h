@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <stdint.h>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -114,6 +115,12 @@ namespace aclb200
 {
 	aclb200_status set_error(aclb200_context* context, aclb200_status status, const std::string& message);
 	aclb200_status check_cuda(aclb200_context* context, cudaError_t error, const char* what);
+	// api.cpp: zeroes *d_out_flags (when given) on the stream, before a launch that ORs ACLB200_ERROR_FLAG_* into it
+	aclb200_status clear_out_flags(aclb200_context* context, uint32_t* d_out_flags, cudaStream_t stream, const char* what);
+	// api.cpp: the pose buffers of a pose operation are rtm::qvvf rows: `pose_stride` (0 on entry: packed rows, set to num_tracks * 48)
+	// holds num_tracks 48 byte bones and keeps them, like every pointer, 16 byte aligned
+	aclb200_status check_qvvf_rows(aclb200_context* context, std::initializer_list<const void*> poses, uint32_t num_tracks, uint64_t& pose_stride,
+		const char* what);
 	// database.cpp: the clip set is bound to a database with at least one chunk streamed in (the launch takes the database kernels)
 	bool database_streamed_in(const aclb200_clipset* clipset);
 
@@ -188,23 +195,20 @@ namespace aclb200
 		float blend_weight;							// the weight when blend_weights == nullptr
 	};
 
-	// the paired decodes of transform_decompress_tracks_kernel: pair r is requests 2r and 2r + 1, combined into output r
-	enum : uint32_t { k_pairs_none = 0, k_pairs_additive = 1, k_pairs_blend = 2 };
+	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
+	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
+	// into output r (aclb200_decompress_tracks_additive / _blend).
+	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_count = 4 };
 
 	// kernels.cu
-	// pairs: a paired decode (additive or blend), planned in whole pairs with both poses of a pair in shared memory
-	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database = false,
-		bool force_output_staging = false, bool pairs = false);
+	// every mode but local assembles its poses in shared memory; additive and blend plan whole pairs
+	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
+		uint32_t compose);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);
-	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t math_mode, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_tracks_object_space(const DecodeParams& params, bool database, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t compose, bool database, cudaStream_t stream);
+	cudaError_t launch_transform_decompress_track(const DecodeParams& params, bool database, cudaStream_t stream);
 	cudaError_t launch_apply_additive(const uint8_t* base_poses, const uint8_t* additive_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream);
-	cudaError_t launch_transform_decompress_tracks_blend(const DecodeParams& params, bool database, cudaStream_t stream);
 	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);

@@ -557,9 +557,10 @@ extern "C"
 			return ACLB200_OK;
 		if (d_local_poses == nullptr || d_object_poses == nullptr || d_parent_indices == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "local_to_object_space: null pose / parent pointer");
-		const uint64_t stride = pose_stride_bytes != 0 ? pose_stride_bytes : uint64_t(num_tracks) * 48;
-		if (stride < uint64_t(num_tracks) * 48 || (stride % 16) != 0 || (reinterpret_cast<uintptr_t>(d_local_poses) % 16) != 0 || (reinterpret_cast<uintptr_t>(d_object_poses) % 16) != 0)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "local_to_object_space: poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
+		uint64_t stride = pose_stride_bytes;
+		aclb200_status status = check_qvvf_rows(context, { d_local_poses, d_object_poses }, num_tracks, stride, "local_to_object_space");
+		if (status != ACLB200_OK)
+			return status;
 
 		ObjectSpaceParams op = {};
 		op.local_poses = static_cast<const uint8_t*>(d_local_poses);
@@ -576,12 +577,9 @@ extern "C"
 
 		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		if (d_out_flags != nullptr)
-		{
-			const cudaError_t cleared = cudaMemsetAsync(d_out_flags, 0, sizeof(uint32_t), cuda_stream);
-			if (cleared != cudaSuccess)
-				return check_cuda(context, cleared, "local_to_object_space");
-		}
+		status = clear_out_flags(context, d_out_flags, cuda_stream, "local_to_object_space");
+		if (status != ACLB200_OK)
+			return status;
 		const uint64_t blocks_needed = (num_poses + warps - 1) / warps;
 		const uint32_t blocks = uint32_t(std::min<uint64_t>(blocks_needed, uint64_t(context->num_sms) * 32));
 		const size_t smem = size_t(warps) * k_object_components * op.plane_stride * sizeof(float);

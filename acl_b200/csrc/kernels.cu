@@ -43,18 +43,19 @@ namespace aclb200
 		//             phase stores its sub-tracks straight to global memory: needed when `skipped` default sub-tracks must keep
 		//             what the caller's buffer holds, or when a pose does not fit in shared memory)
 		// DB        : the clip set's bound database has chunks streamed in: key frames may come from its tier buffers
-		// OBJECT    : the staged poses are taken to object space before they leave (aclb200_decompress_tracks_object_space; OUT_STAGED, QVV48)
-		// PAIR      : k_pairs_additive or k_pairs_blend: requests 2r and 2r + 1 are the two halves of pair r (OUT_STAGED, whole pairs per
-		//             block); phase 4c combines the two rows into row 2r, which is taken to object space when parents are given
-		//             (p.parent_indices, a run-time branch) and leaves as output r.
+		// COMPOSE   : every mode but k_compose_local needs OUT_STAGED.
+		//             k_compose_object: the staged poses are taken to object space before they leave (aclb200_decompress_tracks_object_space, QVV48)
+		//             k_compose_additive, k_compose_blend: requests 2r and 2r + 1 are the two halves of pair r (whole pairs per block); phase 4c
+		//             combines the two rows into row 2r, which is taken to object space when parents are given (p.parent_indices, a run-time
+		//             branch) and leaves as output r.
 		//             additive (aclb200_decompress_tracks_additive): base and additive half; the additive half takes the track_writer defaults.
 		//             blend (aclb200_decompress_tracks_blend): from and to half, both full poses; row 2r becomes rtm::qvv_lerp(from, to, weight).
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB = false, bool OBJECT = false, uint32_t PAIR = k_pairs_none>
+		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
-			constexpr bool PAIRED = PAIR != k_pairs_none;
-			static_assert(!PAIRED || (OUT_STAGED && !OBJECT), "the paired decodes combine poses assembled in shared memory");
+			constexpr bool PAIRED = COMPOSE == k_compose_additive || COMPOSE == k_compose_blend;
+			static_assert(COMPOSE == k_compose_local || OUT_STAGED, "the composed decodes work on poses assembled in shared memory");
 			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
 			// dynamic shared memory: RS[requests_per_block] | key frame windows | pose staging
 			extern __shared__ __align__(16) uint8_t s_dynamic[];
@@ -118,7 +119,7 @@ namespace aclb200
 					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
 					uint8_t* pose = OUT_STAGED ? s_out + size_t(local_request) * p.smem_pose_bytes : rs.out;
 					constant_sub_tracks<NORM, false>(p, rs, bone, desc, pose + size_t(bone) * p.bone_stride,
-						PAIR == k_pairs_additive && (local_request & 1u) != 0);
+						COMPOSE == k_compose_additive && (local_request & 1u) != 0);
 				}
 			}
 
@@ -174,7 +175,7 @@ namespace aclb200
 
 			// ---- phase 4c: one thread per (pair, bone) applies the additive row (request 2r + 1) to the base row (request 2r), in place;
 			// a pair whose halves differ in bone count (or name an invalid clip) is left alone and never stored ----
-			if constexpr (PAIR == k_pairs_additive)
+			if constexpr (COMPOSE == k_compose_additive)
 			{
 				__syncthreads();
 				uint32_t flags = 0;
@@ -203,7 +204,7 @@ namespace aclb200
 
 			// ---- phase 4c, blend: one thread per (pair, bone) lerps the from row (request 2r) towards the to row (request 2r + 1), in place,
 			// with the pair's weight; pairs whose halves differ in bone count are left alone as above ----
-			if constexpr (PAIR == k_pairs_blend)
+			if constexpr (COMPOSE == k_compose_blend)
 			{
 				__syncthreads();
 				const uint32_t first_pair = first_request >> 1;
@@ -223,9 +224,8 @@ namespace aclb200
 
 			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (PAIRED: the
 			// combined row of each pair, when parents are given) ----
-			if constexpr (OBJECT || PAIRED)
+			if constexpr (COMPOSE != k_compose_local)
 			{
-				static_assert(OUT_STAGED, "the object space walk runs on poses assembled in shared memory");
 				if (!PAIRED || p.parent_indices != nullptr)
 				{
 					__syncthreads();
@@ -786,45 +786,42 @@ namespace aclb200
 			return divisor <= 1 ? 0u : uint32_t((uint64_t(1) << 32) / divisor) + 1u;
 		}
 
-		template<int NORM, bool PER_TRACK, bool DB = false>
-		cudaError_t launch_tracks(const DecodeParams& params, cudaStream_t stream)
+		using DecodeKernel = void (*)(DecodeParams);
+
+		// f(std::integral_constant<uint32_t, value>) for a run-time value < N, f(std::bool_constant<value>) for a run-time bool
+		template<uint32_t N, typename F>
+		DecodeKernel with_constant(uint32_t value, F f)
 		{
-			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
-			const bool staged = params.stage_bytes != 0;
-			const bool out_staged = params.smem_pose_bytes != 0;
-			if (staged && out_staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			else if (staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, false, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			else if (out_staged)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+			if constexpr (N == 1)
+				return f(std::integral_constant<uint32_t, 0>());
 			else
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, false, DB><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			return cudaGetLastError();
+				return value == N - 1 ? f(std::integral_constant<uint32_t, N - 1>()) : with_constant<N - 1>(value, f);
 		}
 
-		// The object space decode: poses are always staged in shared memory, key frames whenever they fit beside them (plan_launch)
-		template<int NORM, bool PER_TRACK, bool DB>
-		cudaError_t launch_tracks_object_space(const DecodeParams& params, cudaStream_t stream)
+		template<typename F>
+		DecodeKernel with_bool(bool value, F f)
 		{
-			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
-			if (params.stage_bytes != 0)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			else
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB, true><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			return cudaGetLastError();
+			return value ? f(std::true_type()) : f(std::false_type());
 		}
 
-		// The paired decodes: params.num_requests = 2 x pairs, params.requests_per_block even (plan_launch(..., pairs = true))
-		template<int NORM, bool PER_TRACK, bool DB, uint32_t PAIR>
-		cudaError_t launch_tracks_pairs(const DecodeParams& params, cudaStream_t stream)
+		// The transform_decompress_tracks_kernel instance of a launch, nullptr for a choice no plan makes: a composed decode always assembles
+		// its poses in shared memory. configure_kernels walks every choice through here, so every kernel a launch can pick is configured.
+		DecodeKernel tracks_kernel(uint32_t normalization, bool per_track, bool database, bool staged, bool out_staged, uint32_t compose)
 		{
-			const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
-			if (params.stage_bytes != 0)
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, true, true, DB, false, PAIR><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			else
-				transform_decompress_tracks_kernel<NORM, PER_TRACK, false, true, DB, false, PAIR><<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
-			return cudaGetLastError();
+			return with_constant<3>(normalization, [&](auto NORM) { return with_bool(per_track, [&](auto PER_TRACK) {
+				return with_bool(database, [&](auto DB) { return with_bool(staged, [&](auto STAGED) { return with_bool(out_staged, [&](auto OUT_STAGED) {
+					return with_constant<k_compose_count>(compose, [&](auto COMPOSE) -> DecodeKernel {
+						if constexpr (COMPOSE != k_compose_local && !OUT_STAGED)
+							return nullptr;
+						else
+							return transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, COMPOSE>;
+					}); }); }); }); }); });
+		}
+
+		DecodeKernel track_kernel(uint32_t normalization, bool per_track, bool database)
+		{
+			return with_constant<3>(normalization, [&](auto NORM) { return with_bool(per_track, [&](auto PER_TRACK) {
+				return with_bool(database, [&](auto DB) -> DecodeKernel { return transform_decompress_track_kernel<NORM, PER_TRACK, DB>; }); }); });
 		}
 
 		// aclb200_apply_additive_to_base: one thread per (pose, bone) of QVV48 rows; out may be either input (a thread reads its two rows
@@ -861,56 +858,11 @@ namespace aclb200
 			}
 		}
 
-		template<int NORM, bool PER_TRACK, bool DB = false>
-		cudaError_t launch_track(const DecodeParams& params, cudaStream_t stream)
+		// the pose operations: one thread per (pose, bone), at most 16 blocks of 256 threads per SM, which loop over the rest
+		uint32_t pose_operation_blocks(uint64_t num_poses, uint32_t num_tracks, int num_sms)
 		{
-			const uint32_t blocks = (params.num_requests + 127) / 128;
-			transform_decompress_track_kernel<NORM, PER_TRACK, DB><<<blocks, 128, 0, stream>>>(params);
-			return cudaGetLastError();
-		}
-
-		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, bool OBJECT = false, uint32_t PAIR = k_pairs_none>
-		cudaError_t set_smem_attribute_one(int optin_limit, int& min_available)
-		{
-			// the opt-in limit covers static + dynamic shared memory
-			cudaFuncAttributes attributes;
-			cudaError_t error = cudaFuncGetAttributes(&attributes, transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, PAIR>);
-			if (error != cudaSuccess)
-				return error;
-			const int available = optin_limit - int(attributes.sharedSizeBytes);
-			if (available < min_available)
-				min_available = available;
-			return cudaFuncSetAttribute(transform_decompress_tracks_kernel<NORM, PER_TRACK, STAGED, OUT_STAGED, DB, OBJECT, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, available);
-		}
-
-		template<int NORM, bool PER_TRACK>
-		cudaError_t set_smem_attribute(int optin_limit, int& min_available)
-		{
-			cudaError_t error = cudaSuccess;
-			for (int db = 0; db < 2 && error == cudaSuccess; ++db)
-			{
-				error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, false, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, false, false>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, false, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, false, false>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, true>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, true>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, true>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, false, k_pairs_additive>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, false, k_pairs_additive>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, false, k_pairs_additive>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, false, k_pairs_additive>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, true, true, true, false, k_pairs_blend>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, true, true, false, false, k_pairs_blend>(optin_limit, min_available);
-				if (error == cudaSuccess) error = db ? set_smem_attribute_one<NORM, PER_TRACK, false, true, true, false, k_pairs_blend>(optin_limit, min_available)
-					: set_smem_attribute_one<NORM, PER_TRACK, false, true, false, false, k_pairs_blend>(optin_limit, min_available);
-			}
-			return error;
+			const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
+			return uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
 		}
 	}
 
@@ -920,12 +872,24 @@ namespace aclb200
 	{
 		const int optin_limit = max_dynamic_smem - 1024;
 		int available = optin_limit;
-		cudaError_t error = set_smem_attribute<0, false>(optin_limit, available);
-		if (error == cudaSuccess) error = set_smem_attribute<0, true>(optin_limit, available);
-		if (error == cudaSuccess) error = set_smem_attribute<1, false>(optin_limit, available);
-		if (error == cudaSuccess) error = set_smem_attribute<1, true>(optin_limit, available);
-		if (error == cudaSuccess) error = set_smem_attribute<2, false>(optin_limit, available);
-		if (error == cudaSuccess) error = set_smem_attribute<2, true>(optin_limit, available);
+		cudaError_t error = cudaSuccess;
+		for (uint32_t choice = 0; choice < 3 * 16 * k_compose_count && error == cudaSuccess; ++choice)
+		{
+			// (normalization, per_track | database << 1 | staged << 2 | out_staged << 3, compose)
+			const uint32_t compose = choice % k_compose_count, bits = choice / k_compose_count % 16, normalization = choice / (16 * k_compose_count);
+			const DecodeKernel kernel = tracks_kernel(normalization, bits & 1, bits & 2, bits & 4, bits & 8, compose);
+			if (kernel == nullptr)
+				continue;
+			// the opt-in limit covers static + dynamic shared memory
+			cudaFuncAttributes attributes;
+			error = cudaFuncGetAttributes(&attributes, kernel);
+			if (error != cudaSuccess)
+				break;
+			const int kernel_available = optin_limit - int(attributes.sharedSizeBytes);
+			if (kernel_available < available)
+				available = kernel_available;
+			error = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kernel_available);
+		}
 		if (error == cudaSuccess) error = configure_pipeline_kernels(optin_limit, available);
 		if (error == cudaSuccess) error = configure_error_kernels(available);
 		max_dynamic_smem = available;
@@ -933,12 +897,14 @@ namespace aclb200
 	}
 
 	// requests_per_block, the division magics and the shared memory carve-up of a launch
-	// force_output_staging: the object space decode needs every pose in shared memory, so a pose that does not fit gives up key frame
-	// staging instead (params.smem_bytes then tells the caller whether one request fits at all)
-	// pairs: requests_per_block stays even, so that the two halves of a pair always share a block
+	// compose != local: the composed decodes need every pose in shared memory, so a pose that does not fit gives up key frame staging
+	// instead (params.smem_bytes then tells the caller whether one request fits at all)
+	// additive, blend: requests_per_block stays even, so that the two halves of a pair always share a block
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
-		bool force_output_staging, bool pairs)
+		uint32_t compose)
 	{
+		const bool force_output_staging = compose != k_compose_local;
+		const bool pairs = compose == k_compose_additive || compose == k_compose_blend;
 		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);
@@ -978,114 +944,38 @@ namespace aclb200
 		params.out_vector16 = ((uint64_t(reinterpret_cast<uintptr_t>(params.out)) | params.pose_stride) & 15) == 0 ? 1u : 0u;
 	}
 
-	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t /*math_mode*/, cudaStream_t stream)
+	// Both math modes run these exact kernels (only the pipeline kernel has a fast variant)
+	cudaError_t launch_transform_decompress_tracks(const DecodeParams& params, uint32_t compose, bool database, cudaStream_t stream)
 	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_tracks<0, true>(params, stream) : launch_tracks<0, false>(params, stream);
-		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_tracks<1, true>(params, stream) : launch_tracks<1, false>(params, stream);
-		default: return per_track ? launch_tracks<2, true>(params, stream) : launch_tracks<2, false>(params, stream);
-		}
+		const DecodeKernel kernel = tracks_kernel(params.normalization, params.per_track_rounding != 0, database, params.stage_bytes != 0,
+			params.smem_pose_bytes != 0, compose);
+		if (kernel == nullptr)
+			return cudaErrorInvalidConfiguration;
+		const uint32_t blocks = (params.num_requests + params.requests_per_block - 1) / params.requests_per_block;
+		kernel<<<blocks, k_threads_per_block, params.smem_bytes, stream>>>(params);
+		return cudaGetLastError();
 	}
 
-	cudaError_t launch_transform_decompress_track(const DecodeParams& params, uint32_t /*math_mode*/, cudaStream_t stream)
+	cudaError_t launch_transform_decompress_track(const DecodeParams& params, bool database, cudaStream_t stream)
 	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_track<0, true>(params, stream) : launch_track<0, false>(params, stream);
-		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_track<1, true>(params, stream) : launch_track<1, false>(params, stream);
-		default: return per_track ? launch_track<2, true>(params, stream) : launch_track<2, false>(params, stream);
-		}
-	}
-
-	// The same launches with the database instances (plan_launch(..., database = true)): both math modes run the exact kernels,
-	// as the plain kernels do
-	cudaError_t launch_transform_decompress_tracks_database(const DecodeParams& params, cudaStream_t stream)
-	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_tracks<0, true, true>(params, stream) : launch_tracks<0, false, true>(params, stream);
-		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_tracks<1, true, true>(params, stream) : launch_tracks<1, false, true>(params, stream);
-		default: return per_track ? launch_tracks<2, true, true>(params, stream) : launch_tracks<2, false, true>(params, stream);
-		}
-	}
-
-	cudaError_t launch_transform_decompress_track_database(const DecodeParams& params, cudaStream_t stream)
-	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER: return per_track ? launch_track<0, true, true>(params, stream) : launch_track<0, false, true>(params, stream);
-		case ACLB200_NORMALIZE_LERP_ONLY: return per_track ? launch_track<1, true, true>(params, stream) : launch_track<1, false, true>(params, stream);
-		default: return per_track ? launch_track<2, true, true>(params, stream) : launch_track<2, false, true>(params, stream);
-		}
-	}
-
-	// The object space decode: both math modes run the exact kernels (the walk is IEEE exact whatever the decode does)
-	cudaError_t launch_transform_decompress_tracks_object_space(const DecodeParams& params, bool database, cudaStream_t stream)
-	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER:
-			return database ? (per_track ? launch_tracks_object_space<0, true, true>(params, stream) : launch_tracks_object_space<0, false, true>(params, stream))
-				: (per_track ? launch_tracks_object_space<0, true, false>(params, stream) : launch_tracks_object_space<0, false, false>(params, stream));
-		case ACLB200_NORMALIZE_LERP_ONLY:
-			return database ? (per_track ? launch_tracks_object_space<1, true, true>(params, stream) : launch_tracks_object_space<1, false, true>(params, stream))
-				: (per_track ? launch_tracks_object_space<1, true, false>(params, stream) : launch_tracks_object_space<1, false, false>(params, stream));
-		default:
-			return database ? (per_track ? launch_tracks_object_space<2, true, true>(params, stream) : launch_tracks_object_space<2, false, true>(params, stream))
-				: (per_track ? launch_tracks_object_space<2, true, false>(params, stream) : launch_tracks_object_space<2, false, false>(params, stream));
-		}
-	}
-
-	// The paired decodes: both math modes run the exact kernels, as the object space decode does
-	template<uint32_t PAIR>
-	cudaError_t launch_transform_decompress_tracks_pairs(const DecodeParams& params, bool database, cudaStream_t stream)
-	{
-		const bool per_track = params.per_track_rounding != 0;
-		switch (params.normalization)
-		{
-		case ACLB200_NORMALIZE_NEVER:
-			return database ? (per_track ? launch_tracks_pairs<0, true, true, PAIR>(params, stream) : launch_tracks_pairs<0, false, true, PAIR>(params, stream))
-				: (per_track ? launch_tracks_pairs<0, true, false, PAIR>(params, stream) : launch_tracks_pairs<0, false, false, PAIR>(params, stream));
-		case ACLB200_NORMALIZE_LERP_ONLY:
-			return database ? (per_track ? launch_tracks_pairs<1, true, true, PAIR>(params, stream) : launch_tracks_pairs<1, false, true, PAIR>(params, stream))
-				: (per_track ? launch_tracks_pairs<1, true, false, PAIR>(params, stream) : launch_tracks_pairs<1, false, false, PAIR>(params, stream));
-		default:
-			return database ? (per_track ? launch_tracks_pairs<2, true, true, PAIR>(params, stream) : launch_tracks_pairs<2, false, true, PAIR>(params, stream))
-				: (per_track ? launch_tracks_pairs<2, true, false, PAIR>(params, stream) : launch_tracks_pairs<2, false, false, PAIR>(params, stream));
-		}
-	}
-
-	cudaError_t launch_transform_decompress_tracks_additive(const DecodeParams& params, bool database, cudaStream_t stream)
-	{
-		return launch_transform_decompress_tracks_pairs<k_pairs_additive>(params, database, stream);
-	}
-
-	cudaError_t launch_transform_decompress_tracks_blend(const DecodeParams& params, bool database, cudaStream_t stream)
-	{
-		return launch_transform_decompress_tracks_pairs<k_pairs_blend>(params, database, stream);
+		const uint32_t blocks = (params.num_requests + 127) / 128;
+		track_kernel(params.normalization, params.per_track_rounding != 0, database)<<<blocks, 128, 0, stream>>>(params);
+		return cudaGetLastError();
 	}
 
 	cudaError_t launch_apply_additive(const uint8_t* base_poses, const uint8_t* additive_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream)
 	{
-		const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
-		const uint32_t blocks = uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
-		apply_additive_kernel<<<blocks, 256, 0, stream>>>(base_poses, additive_poses, out, num_poses, num_tracks, pose_stride, additive_format, flags);
+		apply_additive_kernel<<<pose_operation_blocks(num_poses, num_tracks, num_sms), 256, 0, stream>>>(base_poses, additive_poses, out, num_poses,
+			num_tracks, pose_stride, additive_format, flags);
 		return cudaGetLastError();
 	}
 
 	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream)
 	{
-		const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
-		const uint32_t blocks = uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
-		blend_poses_kernel<<<blocks, 256, 0, stream>>>(from_poses, to_poses, out, num_poses, num_tracks, pose_stride, weight, weights);
+		blend_poses_kernel<<<pose_operation_blocks(num_poses, num_tracks, num_sms), 256, 0, stream>>>(from_poses, to_poses, out, num_poses, num_tracks,
+			pose_stride, weight, weights);
 		return cudaGetLastError();
 	}
 

@@ -1,8 +1,8 @@
 // acl_b200/csrc/object_space.cuh -- the hierarchy walk shared by the error measurement (error_metric.cu: object_space_kernel) and the
-// object space decode (kernels.cu: transform_decompress_tracks_kernel<..., OBJECT = true>): the reference's qvv and 3x4 matrix operations
-// restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which the
-// error measurement, the additive decode (PAIR = k_pairs_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which the
-// blend decode (PAIR = k_pairs_blend) and aclb200_blend_poses share.
+// object space decode (kernels.cu: transform_decompress_tracks_kernel<..., COMPOSE = k_compose_object>): the reference's qvv and 3x4 matrix
+// operations restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which
+// the error measurement, the additive decode (COMPOSE = k_compose_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which
+// the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share.
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
