@@ -163,6 +163,10 @@ def _lib():
         l.aclb200_apply_additive_to_base.argtypes = [vp, vp, vp, vp, u64, u32, u64, u32, vp, vp]
         l.aclb200_decompress_tracks_blend.argtypes = [vp, vp, vp, u32, C.POINTER(Options), C.c_float, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_blend_poses.argtypes = [vp, vp, vp, vp, u64, u32, u64, C.c_float, vp, vp]
+        l.aclb200_decompress_tracks_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, vp, vp, vp, vp]
+        l.aclb200_decompress_tracks_additive_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), u32, vp, vp, vp, vp, vp, vp, vp]
+        l.aclb200_decompress_tracks_blend_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), C.c_float, vp, vp, vp, vp, vp, vp, vp]
+        l.aclb200_local_to_skinning.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -190,7 +194,8 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_all_samples", "aclb200_upload_database", "aclb200_release_database", "aclb200_database_get_info",
         "aclb200_database_get_loaded_chunks", "aclb200_database_stream_in", "aclb200_database_stream_out", "aclb200_clipset_bind_database",
         "aclb200_decompress_tracks_object_space", "aclb200_decompress_tracks_additive", "aclb200_apply_additive_to_base",
-        "aclb200_decompress_tracks_blend", "aclb200_blend_poses",
+        "aclb200_decompress_tracks_blend", "aclb200_blend_poses", "aclb200_decompress_tracks_skinning",
+        "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
     ]
 
 
@@ -440,6 +445,45 @@ class Context:
                                                            C.byref(options), weight, _device_ptr(d_weights), _device_ptr(d_parent_indices),
                                                            _device_ptr(d_skeleton_offsets), kind, _device_ptr(d_out), _device_ptr(d_out_flags),
                                                            _stream_ptr(stream)))
+
+    # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
+    # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as
+    # three float4 rows, row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]) of the skinning matrix: skinned[c] = dot(row c, (p, 1)). ----
+    def decompress_tracks_skinning(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices, d_inverse_bind,
+                                   d_out, d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_object_space(OBJECT_MATRIX3X4F) followed by the skinning step, in one kernel; clip c uses the skeleton and the
+        inverse binds at offset d_skeleton_offsets[c] (None: 0)."""
+        self._check(_lib().aclb200_decompress_tracks_skinning(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
+                                                              _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                              _device_ptr(d_inverse_bind), _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                              _stream_ptr(stream)))
+
+    def decompress_tracks_additive_skinning(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices,
+                                            d_inverse_bind, d_out, additive_format: int = 0, d_clip_additive_formats=None,
+                                            d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_additive's combined poses as skinning rows, with the base clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_additive_skinning(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                       C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
+                                                                       _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                                       _device_ptr(d_inverse_bind), _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                                       _stream_ptr(stream)))
+
+    def decompress_tracks_blend_skinning(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices,
+                                         d_inverse_bind, d_out, weight: float = 0.5, d_weights=None, d_skeleton_offsets=None,
+                                         d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_blend's blended poses as skinning rows, with the from clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_blend_skinning(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                    C.byref(options), weight, _device_ptr(d_weights), _device_ptr(d_parent_indices),
+                                                                    _device_ptr(d_skeleton_offsets), _device_ptr(d_inverse_bind), _device_ptr(d_out),
+                                                                    _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def local_to_skinning(self, d_local_poses, d_out, num_poses: int, num_tracks: int, d_parent_indices, d_inverse_bind,
+                          pose_stride_bytes: int = 0, d_out_flags=None, stream=None) -> None:
+        """Skinning rows of num_poses QVV48 local poses of one skeleton already on the device (skeleton and inverse binds at offset 0),
+        bit-identical to decompress_tracks_skinning; d_out may be d_local_poses."""
+        self._check(_lib().aclb200_local_to_skinning(self._handle, _device_ptr(d_local_poses), _device_ptr(d_out), num_poses, num_tracks,
+                                                     pose_stride_bytes, _device_ptr(d_parent_indices), _device_ptr(d_inverse_bind),
+                                                     _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     def decompress_track(self, clipset: ClipSet, d_requests, d_track_indices, num_requests: int, options: Options, d_out, stream=None) -> None:
         self._check(_lib().aclb200_decompress_track(self._handle, clipset._handle, _device_ptr(d_requests), _device_ptr(d_track_indices),

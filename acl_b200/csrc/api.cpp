@@ -28,6 +28,8 @@ namespace aclb200
 		// the C entry point of each compose mode, for messages
 		const char* const k_compose_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_object_space", "decompress_tracks_additive",
 			"decompress_tracks_blend" };
+		const char* const k_skinning_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_skinning", "decompress_tracks_additive_skinning",
+			"decompress_tracks_blend_skinning" };
 
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
@@ -126,19 +128,22 @@ namespace aclb200
 			return check_cuda(context, error, what);
 		}
 
-		// The composed decodes. Every refusal comes before the flags are cleared: a refused call writes nothing.
+		// The composed decodes. Every refusal comes before the flags are cleared: a refused call writes nothing. d_inverse_bind is given by
+		// the skinning entry points only (they require parents), and makes the object kind k_object_skinning.
 		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, uint32_t compose, const uint32_t* d_parent_indices,
-			const uint32_t* d_skeleton_offsets, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream,
+			const uint32_t* d_skeleton_offsets, const float* d_inverse_bind, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream,
 			const std::function<void(DecodeParams&)>& set_pair_operands = nullptr)
 		{
-			const std::string entry = k_compose_entry[compose];
+			const std::string entry = d_inverse_bind != nullptr ? k_skinning_entry[compose] : k_compose_entry[compose];
 			DecodeParams params;
 			const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, compose);
 			if (status != ACLB200_OK)
 				return status;
 			// object space output: always in the object space decode (its entry point requires parents), with parents in the paired ones
-			if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+			if (d_inverse_bind != nullptr)
+				object_kind = k_object_skinning;
+			else if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": unknown object_kind");
 			if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
@@ -152,6 +157,7 @@ namespace aclb200
 			params.skeleton_offsets = d_skeleton_offsets;
 			params.object_flags = d_out_flags;
 			params.object_kind = object_kind;
+			params.inverse_bind = d_inverse_bind;
 			if (set_pair_operands)
 				set_pair_operands(params);
 			cudaSetDevice(context->device);
@@ -180,6 +186,24 @@ namespace aclb200
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": poses are rtm::qvvf rows (48 byte bones), 16 byte aligned");
 		return ACLB200_OK;
 	}
+
+	aclb200_status check_inverse_binds(aclb200_context* context, const float* d_inverse_bind, const char* what)
+	{
+		if (d_inverse_bind == nullptr || (reinterpret_cast<uintptr_t>(d_inverse_bind) % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": inverse binds are 12 float matrices, 16 byte aligned, never NULL");
+		return ACLB200_OK;
+	}
+
+	namespace
+	{
+		// what the three skinning decodes check of their own before the composed path: parents and inverse binds
+		aclb200_status check_skinning_operands(aclb200_context* context, const uint32_t* d_parent_indices, const float* d_inverse_bind, const char* what)
+		{
+			if (d_parent_indices == nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": null parent index pointer");
+			return check_inverse_binds(context, d_inverse_bind, what);
+		}
+	}
 }
 
 using namespace aclb200;
@@ -188,7 +212,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.8 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.9 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -394,7 +418,19 @@ extern "C"
 		if (d_parent_indices == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: null parent index pointer");
 		return decompress_composed(context, clipset, d_requests, num_requests, options, k_compose_object, d_parent_indices, d_skeleton_offsets,
-			object_kind, d_out, d_out_flags, stream);
+			nullptr, object_kind, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_tracks_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		return decompress_composed(context, clipset, d_requests, num_requests, options, k_compose_object, d_parent_indices, d_skeleton_offsets,
+			d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
@@ -410,7 +446,28 @@ extern "C"
 		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
 		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
 		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_additive,
-			d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			{
+				params.additive_format = additive_format;
+				params.clip_additive_formats = d_clip_additive_formats;
+			});
+	}
+
+	aclb200_status aclb200_decompress_tracks_additive_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		if (num_requests > 0x7FFFFFFFu)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive_skinning: more than 2^31 - 1 pairs");
+		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive_skinning: additive_format out of range");
+		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_additive_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_additive,
+			d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream, [&](DecodeParams& params)
 			{
 				params.additive_format = additive_format;
 				params.clip_additive_formats = d_clip_additive_formats;
@@ -455,7 +512,26 @@ extern "C"
 		static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
 			"a blend request is two requests back to back");
 		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_blend,
-			d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			{
+				params.blend_weight = weight;
+				params.blend_weights = d_weights;
+			});
+	}
+
+	aclb200_status aclb200_decompress_tracks_blend_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		float weight, const float* d_weights,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		if (num_requests > 0x7FFFFFFFu)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend_skinning: more than 2^31 - 1 pairs");
+		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_blend_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_blend,
+			d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream, [&](DecodeParams& params)
 			{
 				params.blend_weight = weight;
 				params.blend_weights = d_weights;
@@ -479,6 +555,33 @@ extern "C"
 		return finish_launch(context, launch_blend_poses(static_cast<const uint8_t*>(d_from_poses), static_cast<const uint8_t*>(d_to_poses),
 			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, weight, d_weights, context->num_sms, static_cast<cudaStream_t>(stream)),
 			"blend_poses");
+	}
+
+	aclb200_status aclb200_local_to_skinning(aclb200_context* context, const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks,
+		uint64_t pose_stride_bytes, const uint32_t* d_parent_indices, const float* d_inverse_bind, uint32_t* d_out_flags, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		if (num_poses == 0 || num_tracks == 0)
+			return ACLB200_OK;
+		if (d_local_poses == nullptr || d_out == nullptr || d_parent_indices == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "local_to_skinning: null pose / parent pointer");
+		uint64_t stride = pose_stride_bytes;
+		aclb200_status status = check_qvvf_rows(context, { d_local_poses, d_out }, num_tracks, stride, "local_to_skinning");
+		if (status == ACLB200_OK)
+			status = check_inverse_binds(context, d_inverse_bind, "local_to_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		const uint32_t warps = local_to_skinning_warps(num_tracks, context->max_dynamic_smem);
+		if (warps == 0)
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, "local_to_skinning: one pose does not fit in a block's shared memory");
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		status = clear_out_flags(context, d_out_flags, cuda_stream, "local_to_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		return finish_launch(context, launch_local_to_skinning(static_cast<const uint8_t*>(d_local_poses), static_cast<uint8_t*>(d_out), num_poses,
+			num_tracks, stride, d_parent_indices, d_inverse_bind, d_out_flags, warps, context->num_sms, cuda_stream), "local_to_skinning");
 	}
 
 	aclb200_status aclb200_decompress_track(aclb200_context* context, const aclb200_clipset* clipset,

@@ -121,6 +121,8 @@ namespace aclb200
 	// holds num_tracks 48 byte bones and keeps them, like every pointer, 16 byte aligned
 	aclb200_status check_qvvf_rows(aclb200_context* context, std::initializer_list<const void*> poses, uint32_t num_tracks, uint64_t& pose_stride,
 		const char* what);
+	// api.cpp: inverse bind matrices are 12 floats per skeleton entry, 16 byte aligned (each lane loads its bone's as three float4)
+	aclb200_status check_inverse_binds(aclb200_context* context, const float* d_inverse_bind, const char* what);
 	// database.cpp: the clip set is bound to a database with at least one chunk streamed in (the launch takes the database kernels)
 	bool database_streamed_in(const aclb200_clipset* clipset);
 
@@ -185,7 +187,8 @@ namespace aclb200
 		const uint32_t* parent_indices;				// skeletons, 0xFFFFFFFF = root
 		const uint32_t* skeleton_offsets;			// [num_clips] first parent index of each clip's skeleton, or nullptr (every clip at 0)
 		uint32_t* object_flags;						// ACLB200_ERROR_FLAG_* are OR-ed in, or nullptr
-		uint32_t object_kind;						// ACLB200_OBJECT_*
+		uint32_t object_kind;						// ACLB200_OBJECT_*, or k_object_skinning (the skinning decodes)
+		const float* inverse_bind;					// k_object_skinning: one 12 float matrix per skeleton entry, in parallel with parent_indices
 		// the additive decode (aclb200_decompress_tracks_additive): requests 2r / 2r + 1 are the base / additive halves of pair r, output r;
 		// parent_indices == nullptr there keeps the combined poses in local space
 		const uint8_t* clip_additive_formats;		// [num_clips] acl::additive_clip_format8 per additive clip (above 3: none), or nullptr
@@ -200,6 +203,10 @@ namespace aclb200
 	// into output r (aclb200_decompress_tracks_additive / _blend).
 	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_count = 4 };
 
+	// The object kind of the skinning decodes (after ACLB200_OBJECT_QVVF and ACLB200_OBJECT_MATRIX3X4F, never taken from a caller): the
+	// matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone, stored as the transposed rows a skinning shader reads
+	constexpr uint32_t k_object_skinning = 2;
+
 	// kernels.cu
 	// every mode but local assembles its poses in shared memory; additive and blend plan whole pairs
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
@@ -211,6 +218,10 @@ namespace aclb200
 		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream);
 	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream);
+	// aclb200_local_to_skinning: one warp per pose, the pose staged in shared memory; 0 warps per block when one pose does not fit
+	uint32_t local_to_skinning_warps(uint32_t num_tracks, int max_dynamic_smem);
+	cudaError_t launch_local_to_skinning(const uint8_t* local_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride,
+		const uint32_t* parents, const float* inverse_bind, uint32_t* flags, uint32_t warps, int num_sms, cudaStream_t stream);
 	cudaError_t launch_transform_debug_seek(const DecodeParams& params, aclb200_seek_state* d_out, cudaStream_t stream);
 	cudaError_t launch_transform_debug_unpack(const DecodeParams& params, uint32_t* d_out, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);

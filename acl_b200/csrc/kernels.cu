@@ -50,6 +50,8 @@ namespace aclb200
 		//             branch) and leaves as output r.
 		//             additive (aclb200_decompress_tracks_additive): base and additive half; the additive half takes the track_writer defaults.
 		//             blend (aclb200_decompress_tracks_blend): from and to half, both full poses; row 2r becomes rtm::qvv_lerp(from, to, weight).
+		//             The object kind k_object_skinning (the _skinning entry points) is a run-time value like the other kinds: the matrix walk,
+		//             then the skinning step of object_space.cuh on the whole pose.
 		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
@@ -236,9 +238,11 @@ namespace aclb200
 						const RS& rs = s_req[local_request];
 						if (rs.num_tracks == 0 || (PAIRED && s_req[local_request + 1].num_tracks != rs.num_tracks))
 							continue;
-						const uint32_t* parents = p.parent_indices + (p.skeleton_offsets != nullptr ? __ldg(p.skeleton_offsets + rs.clip) : 0u);
-						flags |= obj::pose_rows_to_object_space(s_out + size_t(local_request) * p.smem_pose_bytes, rs.num_tracks, parents,
-							p.object_kind == ACLB200_OBJECT_MATRIX3X4F);
+						const uint32_t skeleton = p.skeleton_offsets != nullptr ? __ldg(p.skeleton_offsets + rs.clip) : 0u;
+						uint8_t* pose = s_out + size_t(local_request) * p.smem_pose_bytes;
+						flags |= obj::pose_rows_to_object_space(pose, rs.num_tracks, p.parent_indices + skeleton, p.object_kind != ACLB200_OBJECT_QVVF);
+						if (p.object_kind == k_object_skinning)
+							obj::skin_pose_rows(pose, rs.num_tracks, p.inverse_bind + size_t(skeleton) * 12);
 					}
 					flags = __reduce_or_sync(0xFFFFFFFFu, flags);
 					if ((threadIdx.x & 31u) == 0 && flags != 0 && p.object_flags != nullptr)
@@ -858,6 +862,38 @@ namespace aclb200
 			}
 		}
 
+		// aclb200_local_to_skinning: one warp per pose. The warp stages the pose's local rows in its share of shared memory with coalesced 16
+		// byte loads, runs the walk and the skinning step the skinning decodes run (so the two routes are bit-identical by construction) and
+		// stores the rows the same way. out may be the input: a warp has read its whole pose before it writes any of it.
+		__global__ void __launch_bounds__(256)
+		local_to_skinning_kernel(const uint8_t* local_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride,
+			const uint32_t* parents, const float* inverse_bind, uint32_t* out_flags)
+		{
+			extern __shared__ __align__(16) uint8_t s_poses[];
+			const uint32_t lane = threadIdx.x & 31u;
+			const uint32_t warps_per_block = blockDim.x >> 5;
+			const uint32_t chunks = num_tracks * 3;		// 16 byte chunks per pose
+			uint4* staged = reinterpret_cast<uint4*>(s_poses) + size_t(threadIdx.x >> 5) * chunks;
+			uint32_t flags = 0;
+			for (uint64_t pose = uint64_t(blockIdx.x) * warps_per_block + (threadIdx.x >> 5); pose < num_poses; pose += uint64_t(gridDim.x) * warps_per_block)
+			{
+				const uint4* src = reinterpret_cast<const uint4*>(local_poses + pose * pose_stride);
+				for (uint32_t chunk = lane; chunk < chunks; chunk += 32)
+					staged[chunk] = src[chunk];
+				__syncwarp();
+				flags |= obj::pose_rows_to_object_space(reinterpret_cast<uint8_t*>(staged), num_tracks, parents, true);
+				obj::skin_pose_rows(reinterpret_cast<uint8_t*>(staged), num_tracks, inverse_bind);
+				__syncwarp();
+				uint4* dst = reinterpret_cast<uint4*>(out + pose * pose_stride);
+				for (uint32_t chunk = lane; chunk < chunks; chunk += 32)
+					dst[chunk] = staged[chunk];
+				__syncwarp();
+			}
+			flags = __reduce_or_sync(0xFFFFFFFFu, flags);
+			if (lane == 0 && flags != 0 && out_flags != nullptr)
+				atomicOr(out_flags, flags);
+		}
+
 		// the pose operations: one thread per (pose, bone), at most 16 blocks of 256 threads per SM, which loop over the rest
 		uint32_t pose_operation_blocks(uint64_t num_poses, uint32_t num_tracks, int num_sms)
 		{
@@ -890,6 +926,7 @@ namespace aclb200
 				available = kernel_available;
 			error = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kernel_available);
 		}
+		if (error == cudaSuccess) error = cudaFuncSetAttribute(local_to_skinning_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin_limit);
 		if (error == cudaSuccess) error = configure_pipeline_kernels(optin_limit, available);
 		if (error == cudaSuccess) error = configure_error_kernels(available);
 		max_dynamic_smem = available;
@@ -976,6 +1013,23 @@ namespace aclb200
 	{
 		blend_poses_kernel<<<pose_operation_blocks(num_poses, num_tracks, num_sms), 256, 0, stream>>>(from_poses, to_poses, out, num_poses, num_tracks,
 			pose_stride, weight, weights);
+		return cudaGetLastError();
+	}
+
+	// up to 8 warps per block, as many as whole poses fit the block's shared memory
+	uint32_t local_to_skinning_warps(uint32_t num_tracks, int max_dynamic_smem)
+	{
+		const uint64_t fit = uint64_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0) / (uint64_t(num_tracks) * 48);
+		return uint32_t(fit < 8 ? fit : 8);
+	}
+
+	cudaError_t launch_local_to_skinning(const uint8_t* local_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride,
+		const uint32_t* parents, const float* inverse_bind, uint32_t* flags, uint32_t warps, int num_sms, cudaStream_t stream)
+	{
+		const uint64_t blocks_needed = (num_poses + warps - 1) / warps;
+		const uint32_t blocks = uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
+		local_to_skinning_kernel<<<blocks, warps * 32, size_t(warps) * num_tracks * 48, stream>>>(local_poses, out, num_poses, num_tracks, pose_stride,
+			parents, inverse_bind, flags);
 		return cudaGetLastError();
 	}
 

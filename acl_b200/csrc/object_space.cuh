@@ -2,7 +2,8 @@
 // object space decode (kernels.cu: transform_decompress_tracks_kernel<..., COMPOSE = k_compose_object>): the reference's qvv and 3x4 matrix
 // operations restated with unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which
 // the error measurement, the additive decode (COMPOSE = k_compose_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which
-// the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share.
+// the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share. And the skinning step, which the three composed decodes (with
+// the internal object kind k_object_skinning) and aclb200_local_to_skinning run after the matrix walk.
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
@@ -520,6 +521,30 @@ namespace aclb200
 					}
 				}
 				return flags;
+			}
+
+			// ---- the skinning step (the skinning decodes and aclb200_local_to_skinning): after pose_rows_to_object_space(..., matrix = true)
+			// has walked the WHOLE pose, row b becomes rtm::matrix_mul(inverse_bind[b], object[b]) (rtm's row vector order: a bind pose
+			// vertex goes into the bone's space, then on to the model). It must not start earlier: a child in a later chunk of 32 bones
+			// reads its parent's object matrix from that row. The inverse binds are the 12 float layout of the matrix rows (x_axis, y_axis,
+			// z_axis, w_axis, xyz each), 16 byte aligned; the result leaves as three float4 rows of the skinning matrix's transpose, row c =
+			// (x_axis[c], y_axis[c], z_axis[c], w_axis[c]), so that dot(row c, (p, 1)) is component c of rtm::matrix_mul_point3(p, skin).
+			// Every lane of the warp calls it; a lane only touches the rows of its own bones ----
+			__device__ __forceinline__ void skin_pose_rows(uint8_t* pose, uint32_t num_tracks, const float* inverse_bind)
+			{
+				const Fp<float> fp{};
+				__syncwarp();
+				for (uint32_t bone = threadIdx.x & 31u; bone < num_tracks; bone += 32)
+				{
+					float4* row = reinterpret_cast<float4*>(pose + size_t(bone) * 48);
+					const float4* bind = reinterpret_cast<const float4*>(inverse_bind + size_t(bone) * 12);
+					const float4 a = __ldg(bind), b = __ldg(bind + 1), c = __ldg(bind + 2);
+					const Mat34<float> inverse = { { { a.x, a.y, a.z }, { a.w, b.x, b.y }, { b.z, b.w, c.x }, { c.y, c.z, c.w } } };
+					const Mat34<float> skin = matrix_mul(fp, inverse, load_matrix_row(row));
+					row[0] = make_float4(skin.m[0][0], skin.m[1][0], skin.m[2][0], skin.m[3][0]);
+					row[1] = make_float4(skin.m[0][1], skin.m[1][1], skin.m[2][1], skin.m[3][1]);
+					row[2] = make_float4(skin.m[0][2], skin.m[1][2], skin.m[2][2], skin.m[3][2]);
+				}
 			}
 
 			// ---- apply_additive_to_base on pose rows (the additive decode and aclb200_apply_additive_to_base): one thread per bone, a row of 48

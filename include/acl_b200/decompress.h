@@ -446,6 +446,38 @@ namespace acl_b200
 			m_device->check(aclb200_blend_poses(m_device->get(), d_from_poses, d_to_poses, d_out, num_poses, num_tracks, pose_stride_bytes, weight,
 				d_weights, stream), "aclb200_blend_poses");
 		}
+		// Skinning rows: the ACLB200_OBJECT_MATRIX3X4F walk, then rtm::matrix_mul(inverse_bind, object) per bone, stored as three float4 rows,
+		// row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]). d_inverse_bind holds 12 floats per skeleton entry, 16 byte aligned, in
+		// parallel with d_parent_indices (aclb200_decompress_tracks_skinning and its additive, blend and standalone forms)
+		void decompress_tracks_skinning(const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind, void* d_out,
+			uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, d_parent_indices,
+				d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_skinning");
+		}
+		void decompress_tracks_additive_skinning(const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			uint32_t additive_format, const uint8_t* d_clip_additive_formats, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+			const float* d_inverse_bind, void* d_out, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_additive_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, additive_format,
+				d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream),
+				"aclb200_decompress_tracks_additive_skinning");
+		}
+		void decompress_tracks_blend_skinning(const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			float weight, const float* d_weights, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_blend_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, weight, d_weights,
+				d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_blend_skinning");
+		}
+		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
+		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
+			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_local_to_skinning(m_device->get(), d_local_poses, d_out, num_poses, num_tracks, pose_stride_bytes, d_parent_indices,
+				d_inverse_bind, d_out_flags, stream), "aclb200_local_to_skinning");
+		}
 		// host buffers in, host buffers out, synchronous
 		void decompress_tracks_host(const aclb200_request* requests, uint32_t num_requests, const aclb200_options& options, void* out, size_t out_bytes)
 		{

@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 8
+#define ACLB200_VERSION_MINOR 9
 
 typedef enum aclb200_status
 {
@@ -502,6 +502,49 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_blend(aclb200_context* cont
  * Refused with ACLB200_ERR_INVALID_ARGUMENT: NULL pointers, misaligned rows. */
 ACLB200_API aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,
 	uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride_bytes, float weight, const float* d_weights, void* stream);
+
+/* Skinning matrices: the pose of aclb200_decompress_tracks_object_space, _additive or _blend taken through the ACLB200_OBJECT_MATRIX3X4F
+ * walk (convert_transforms + local_to_object_space of qvvf_matrix3x4f_transform_error_metric, transform_error_metrics.h:397-436; never the
+ * qvvf walk, so no quat_normalize), then per bone
+ *     skin[b] = rtm::matrix_mul(inverse_bind[b], object[b])       (matrix3x4f.h:298-321, rtm's row vector order)
+ * in one kernel: the local and object rows never leave shared memory. Every step is an IEEE multiply or add in the reference's order, so
+ * wherever the route's matrix rows are bit-identical to the reference, so are its skinning rows.
+ *   d_inverse_bind   device, 16 byte aligned: one rtm::matrix3x4f per skeleton entry, in parallel with d_parent_indices (clip c, bone b reads
+ *                    d_inverse_bind + 12 * (d_skeleton_offsets[c] + b)), as the xyz lanes of x_axis, y_axis, z_axis, w_axis (the 12 floats
+ *                    ACLB200_OBJECT_MATRIX3X4F writes). A bone that is not skinned takes the identity.
+ *   d_out            48 bytes per bone, three float4 rows: row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]) of skin, so that component
+ *                    c of rtm::matrix_mul_point3(p, skin) is dot(row c, (p, 1)): what a skinning shader reads. Stride, alignment, invalid
+ *                    clips and pairs, and bytes past num_tracks * 48 as the entry point each call mirrors.
+ *   d_out_flags      as that entry point: ACLB200_ERROR_FLAG_INVALID_SKELETON from the walk, ACLB200_ERROR_FLAG_NEGATIVE_SCALE from an
+ *                    additive `relative` bone that took qvv_mul's matrix branch (the matrix walk itself has no branch)
+ * The skeleton and the inverse binds are those of the base clip (additive) or of the from clip (blend).
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, writing nothing: NULL parents or inverse binds, a d_inverse_bind that is not 16 byte aligned,
+ * skip masks or a `skipped` default mode, an output layout other than QVV48, a scalar clip set, additive_format > 3, an output that breaks
+ * the alignment rules of aclb200_decompress_tracks. ACLB200_ERR_UNSUPPORTED when a pose (or a pair) does not fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+ACLB200_API aclb200_status aclb200_decompress_tracks_additive_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_additive_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+ACLB200_API aclb200_status aclb200_decompress_tracks_blend_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	float weight, const float* d_weights,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
+ * aclb200_apply_additive_to_base): num_poses poses of rtm::qvvf rows of one skeleton (48 byte bones, 16 byte aligned, pose p at
+ * p * pose_stride_bytes in both buffers, 0 = num_tracks * 48) in, skinning rows out, bit-identical to the fused route. The skeleton is
+ * d_parent_indices and the inverse binds d_inverse_bind, both at offset 0. d_out may be d_local_poses. d_out_flags as
+ * aclb200_local_to_object_space. Refused with ACLB200_ERR_INVALID_ARGUMENT: NULL pointers, misaligned rows or inverse binds;
+ * ACLB200_ERR_UNSUPPORTED when one pose does not fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_local_to_skinning(aclb200_context* context, const void* d_local_poses, void* d_out, uint64_t num_poses,
+	uint32_t num_tracks, uint64_t pose_stride_bytes, const uint32_t* d_parent_indices, const float* d_inverse_bind, uint32_t* d_out_flags,
+	void* stream);
 
 /* Parity / debugging hooks (integer stages of the decode, bit-exact against the reference):
  *  - aclb200_debug_seek: the state seek_v0 computes, one aclb200_seek_state per request (device output).

@@ -114,6 +114,31 @@ for parents in (None, d_parents):
         bad += not clips.bit_equal(got[i, :counts[c]][:, L], want[:, L])
 ctx.blend_poses(out, out, out, len(blend_pairs), cs.max_tracks, d_weights=d_blend_weights)
 torch.cuda.synchronize()
+# skinning decodes: the object, additive and blend instances with the skinning step (per clip skeletons and inverse binds), and the
+# standalone local_to_skinning_kernel, in place
+from oracle import skinning
+from tests import skinning_cases
+inverses = [skinning_cases.random_affine(int(counts[c]), c, mirrored=True) for c in range(len(names))]
+d_inverse = torch.from_numpy(np.concatenate(inverses)).cuda()
+out = torch.zeros((len(req), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+ctx.decompress_tracks_skinning(cs, d_req, len(req), ab.Options(), d_parents, d_inverse, out, d_skeleton_offsets=d_offsets)
+torch.cuda.synchronize()
+got = out.cpu().numpy()
+for i in range(0, len(req), 7):
+    c = req_clip[i]
+    local = port.transform_decompress_tracks(blobs[c], settings, float(req_time[i]))
+    bad += not clips.bit_equal(got[i, :counts[c]], skinning.port_local_to_skinning(local, trees[c], inverses[c]))
+out = torch.zeros((len(pairs), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+ctx.decompress_tracks_additive_skinning(cs, d_pairs, len(pairs), ab.Options(), d_parents, d_inverse, out, d_clip_additive_formats=d_formats,
+                                        d_skeleton_offsets=d_offsets)
+ctx.decompress_tracks_blend_skinning(cs, d_blend_pairs, len(blend_pairs), ab.Options(), d_parents, d_inverse, out, d_weights=d_blend_weights,
+                                     d_skeleton_offsets=d_offsets)
+one = ctx.upload([blobs[0]])
+local = torch.zeros((64, one.max_tracks, 12), dtype=torch.float32, device="cuda")
+ctx.decompress_tracks(one, torch.from_numpy(ab.make_requests(np.zeros(64), np.linspace(0, 1, 64)).view(np.uint8)).cuda(), 64, ab.Options(), local)
+ctx.local_to_skinning(local, local, 64, one.max_tracks, d_parents, d_inverse)
+torch.cuda.synchronize()
+one.release()
 # scalar clips
 for name in ("float1", "float3", "vector4", "float1_c4_small"):
     blob = clips.load_blob(name); spec = clips.SCALAR_SPECS[name]
