@@ -167,6 +167,8 @@ def _lib():
         l.aclb200_decompress_tracks_additive_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), u32, vp, vp, vp, vp, vp, vp, vp]
         l.aclb200_decompress_tracks_blend_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), C.c_float, vp, vp, vp, vp, vp, vp, vp]
         l.aclb200_local_to_skinning.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp, vp]
+        l.aclb200_decompress_tracks_layered.argtypes = [vp, vp, vp, u32, u32, C.POINTER(Options), u32, vp, vp, vp, u32, vp, vp, vp]
+        l.aclb200_decompress_tracks_layered_skinning.argtypes = [vp, vp, vp, u32, u32, C.POINTER(Options), u32, vp, vp, vp, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -196,6 +198,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_object_space", "aclb200_decompress_tracks_additive", "aclb200_apply_additive_to_base",
         "aclb200_decompress_tracks_blend", "aclb200_blend_poses", "aclb200_decompress_tracks_skinning",
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
+        "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
     ]
 
 
@@ -234,6 +237,24 @@ def make_blend_requests(from_clips, from_times, to_clips, to_times) -> np.ndarra
     out["from_time"] = np.asarray(from_times, dtype=np.float32)
     out["to_clip"] = np.asarray(to_clips, dtype=np.uint32)
     out["to_time"] = np.asarray(to_times, dtype=np.float32)
+    return out
+
+
+LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE = 0, 1, 2
+MAX_LAYERS = 8
+LAYER_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("op", np.uint32), ("weight", np.float32)])
+
+
+def make_layers(clips, times, ops, weights) -> np.ndarray:
+    """[num_poses][num_layers] arrays (or anything that broadcasts to one shape) of clip, sample time, LAYER_* op and blend weight ->
+    aclb200_layer[num_poses][num_layers]; pose r's layers are row r."""
+    clips, times, ops, weights = np.broadcast_arrays(np.asarray(clips, dtype=np.uint32), np.asarray(times, dtype=np.float32),
+                                                     np.asarray(ops, dtype=np.uint32), np.asarray(weights, dtype=np.float32))
+    out = np.empty(clips.shape, dtype=LAYER_DTYPE)
+    out["clip"] = clips
+    out["sample_time"] = times
+    out["op"] = ops
+    out["weight"] = weights
     return out
 
 
@@ -446,6 +467,21 @@ class Context:
                                                            _device_ptr(d_skeleton_offsets), kind, _device_ptr(d_out), _device_ptr(d_out_flags),
                                                            _stream_ptr(stream)))
 
+    def decompress_tracks_layered(self, clipset: ClipSet, d_layers, num_poses: int, num_layers: int, options: Options, d_out,
+                                  additive_format: int = 0, d_clip_additive_formats=None, d_parent_indices=None, kind: int = 0,
+                                  d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """num_poses stacks of num_layers layers (make_layers, 1..8 per pose). The first layer whose op is not LAYER_OFF is the base,
+        decoded as decompress_tracks decodes it; each later layer is folded into the running pose in order: LAYER_BLEND =
+        rtm::qvv_lerp(running, layer, weight), LAYER_ADDITIVE = apply_additive_to_base(format, running, layer) with the layer decoded with
+        the track_writer defaults (format: d_clip_additive_formats[layer clip], uint8, None: additive_format), LAYER_OFF = not read. With
+        d_parent_indices the running pose leaves in object space as `kind` rows (OBJECT_*), the base clip c's skeleton at d_parent_indices +
+        d_skeleton_offsets[c]; without, in options.output_layout. A pose with an invalid clip, a track count that differs from the base's
+        or an unknown op writes nothing. d_out_flags: optional uint32 ERROR_FLAG_*."""
+        self._check(_lib().aclb200_decompress_tracks_layered(self._handle, clipset._handle, _device_ptr(d_layers), num_poses, num_layers,
+                                                             C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
+                                                             _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
+                                                             _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as
     # three float4 rows, row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]) of the skinning matrix: skinned[c] = dot(row c, (p, 1)). ----
@@ -476,6 +512,16 @@ class Context:
                                                                     C.byref(options), weight, _device_ptr(d_weights), _device_ptr(d_parent_indices),
                                                                     _device_ptr(d_skeleton_offsets), _device_ptr(d_inverse_bind), _device_ptr(d_out),
                                                                     _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def decompress_tracks_layered_skinning(self, clipset: ClipSet, d_layers, num_poses: int, num_layers: int, options: Options,
+                                           d_parent_indices, d_inverse_bind, d_out, additive_format: int = 0, d_clip_additive_formats=None,
+                                           d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_layered's running poses as skinning rows, with the base clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_layered_skinning(self._handle, clipset._handle, _device_ptr(d_layers), num_poses, num_layers,
+                                                                      C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
+                                                                      _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                                      _device_ptr(d_inverse_bind), _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                                      _stream_ptr(stream)))
 
     def local_to_skinning(self, d_local_poses, d_out, num_poses: int, num_tracks: int, d_parent_indices, d_inverse_bind,
                           pose_stride_bytes: int = 0, d_out_flags=None, stream=None) -> None:

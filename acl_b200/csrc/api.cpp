@@ -27,13 +27,17 @@ namespace aclb200
 
 		// the C entry point of each compose mode, for messages
 		const char* const k_compose_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_object_space", "decompress_tracks_additive",
-			"decompress_tracks_blend" };
+			"decompress_tracks_blend", "decompress_tracks_layered" };
 		const char* const k_skinning_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_skinning", "decompress_tracks_additive_skinning",
-			"decompress_tracks_blend_skinning" };
+			"decompress_tracks_blend_skinning", "decompress_tracks_layered_skinning" };
+		// what a composed decode that does not fit one block is refused with
+		const char* const k_unfit_message[k_compose_count] = { "", ": one pose does not fit in a block's shared memory",
+			": the two poses of a pair do not fit in a block's shared memory", ": the two poses of a pair do not fit in a block's shared memory",
+			": the poses of a layer stack do not fit in a block's shared memory" };
 
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			uint32_t compose = k_compose_local)
+			uint32_t compose = k_compose_local, uint32_t num_layers = 1)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -117,6 +121,7 @@ namespace aclb200
 			if (compose != k_compose_local && keeps_bytes)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(k_compose_entry[compose])
 					+ ": the composed poses need every decoded sub-track (no skip masks, no `skipped` default mode)");
+			params.num_layers = num_layers;
 			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !keeps_bytes, database, compose);
 			return ACLB200_OK;
 		}
@@ -133,11 +138,12 @@ namespace aclb200
 		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, uint32_t compose, const uint32_t* d_parent_indices,
 			const uint32_t* d_skeleton_offsets, const float* d_inverse_bind, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream,
-			const std::function<void(DecodeParams&)>& set_pair_operands = nullptr)
+			const std::function<void(DecodeParams&)>& set_pair_operands = nullptr, uint32_t num_layers = 1)
 		{
 			const std::string entry = d_inverse_bind != nullptr ? k_skinning_entry[compose] : k_compose_entry[compose];
 			DecodeParams params;
-			const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, compose);
+			const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, compose,
+				num_layers);
 			if (status != ACLB200_OK)
 				return status;
 			// object space output: always in the object space decode (its entry point requires parents), with parents in the paired ones
@@ -149,8 +155,7 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
 			// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
 			if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + (compose == k_compose_object ? ": one pose does not fit in a block's shared memory"
-					: ": the two poses of a pair do not fit in a block's shared memory"));
+				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + k_unfit_message[compose]);
 			if (num_requests == 0)
 				return ACLB200_OK;
 			params.parent_indices = d_parent_indices;
@@ -203,6 +208,18 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": null parent index pointer");
 			return check_inverse_binds(context, d_inverse_bind, what);
 		}
+
+		// what the two layered decodes check of their own: the stack depth, the launch's request count and the additive format
+		aclb200_status check_layers(aclb200_context* context, uint32_t num_poses, uint32_t num_layers, uint32_t additive_format, const char* what)
+		{
+			if (num_layers == 0 || num_layers > k_max_layers)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": num_layers must be 1 to 8");
+			if (uint64_t(num_poses) * num_layers > 0xFFFFFFFFu)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": num_poses * num_layers is above 2^32 - 1");
+			if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": additive_format out of range");
+			return ACLB200_OK;
+		}
 	}
 }
 
@@ -212,7 +229,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.9 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.10 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -536,6 +553,45 @@ extern "C"
 				params.blend_weight = weight;
 				params.blend_weights = d_weights;
 			});
+	}
+
+	aclb200_status aclb200_decompress_tracks_layered(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		const aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, "decompress_tracks_layered");
+		if (status != ACLB200_OK)
+			return status;
+		// stack r is the requests r L .. r L + L - 1 of the launch, read as layer records by the kernel
+		static_assert(sizeof(aclb200_layer) == 16 && offsetof(aclb200_layer, pose) == 0, "a layer is a request, its op and its weight");
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_layers), num_poses * num_layers, options,
+			k_compose_layers, d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
+			{
+				params.additive_format = additive_format;
+				params.clip_additive_formats = d_clip_additive_formats;
+			}, num_layers);
+	}
+
+	aclb200_status aclb200_decompress_tracks_layered_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, "decompress_tracks_layered_skinning");
+		if (status == ACLB200_OK)
+			status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_layered_skinning");
+		if (status != ACLB200_OK)
+			return status;
+		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_layers), num_poses * num_layers, options,
+			k_compose_layers, d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream,
+			[&](DecodeParams& params)
+			{
+				params.additive_format = additive_format;
+				params.clip_additive_formats = d_clip_additive_formats;
+			}, num_layers);
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

@@ -196,19 +196,29 @@ namespace aclb200
 		// the blend decode (aclb200_decompress_tracks_blend): requests 2r / 2r + 1 are the from / to halves of pair r, output r
 		const float* blend_weights;					// [pairs] the weight of each pair, or nullptr
 		float blend_weight;							// the weight when blend_weights == nullptr
+		// the layered decode (aclb200_decompress_tracks_layered): `requests` holds aclb200_layer records, requests r L .. r L + L - 1 are
+		// the layers of output r (additive_format and clip_additive_formats as above)
+		uint32_t num_layers;						// L, 1..k_max_layers
+		uint32_t magic_layers;						// division_magic(L), for block-local indices
 	};
 
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
-	// into output r (aclb200_decompress_tracks_additive / _blend).
-	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_count = 4 };
+	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
+	// (aclb200_decompress_tracks_layered).
+	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_layers = 4,
+		k_compose_count = 5 };
+
+	// the deepest layer stack of aclb200_decompress_tracks_layered
+	constexpr uint32_t k_max_layers = 8;
 
 	// The object kind of the skinning decodes (after ACLB200_OBJECT_QVVF and ACLB200_OBJECT_MATRIX3X4F, never taken from a caller): the
 	// matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone, stored as the transposed rows a skinning shader reads
 	constexpr uint32_t k_object_skinning = 2;
 
 	// kernels.cu
-	// every mode but local assembles its poses in shared memory; additive and blend plan whole pairs
+	// every mode but local assembles its poses in shared memory; additive and blend plan whole pairs, layers whole stacks of
+	// params.num_layers requests
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
 		uint32_t compose);
 	void plan_scalar_launch(DecodeParams& params, uint32_t max_key_frame_bytes);

@@ -217,14 +217,13 @@ namespace aclb200
 
 		// seek_v0 for transform clips, decompression.transform.h:206-563. DB == false: no database bound (a clip bound to one decodes
 		// from its resident key frames, as a context initialised without the database does). DB == true: the tier branches with the
-		// clip set's bound database (RS = ReqStateDB). PAIRED: requests 2r and 2r + 1 are the two halves of pair r (additive or blend), sharing the
-		// per request policies of pair r.
-		template<bool DB = false, class RS = ReqState, bool PAIRED = false>
-		__device__ __forceinline__ void seek_transform(const DecodeParams& p, uint32_t request_index, RS& rs)
+		// clip set's bound database (RS = ReqStateDB). `policy_index` picks the request's entry of p.request_policies (the composed decodes
+		// share one entry between the requests of an output).
+		template<bool DB = false, class RS = ReqState>
+		__device__ __forceinline__ void seek_request(const DecodeParams& p, const aclb200_request request, uint32_t policy_index, RS& rs)
 		{
 			rs.num_tracks = 0;
 			rs.sample_time = -1.0f;
-			const aclb200_request request = p.requests[request_index];
 			if (request.clip >= p.num_clips)
 				return;
 			const ClipDesc& clip = p.clips[request.clip];
@@ -235,7 +234,7 @@ namespace aclb200
 
 			uint32_t rounding_policy, requested_looping, looping_policy;
 			float duration;
-			request_policies(p, PAIRED ? request_index >> 1 : request_index, rounding_policy, requested_looping);
+			request_policies(p, policy_index, rounding_policy, requested_looping);
 			resolve_looping(p, clip, requested_looping, looping_policy, duration);
 
 			float sample_time = request.sample_time;
@@ -405,6 +404,14 @@ namespace aclb200
 					rs.bit_base[1] = rs.kf_bit[1];
 				}
 			}
+		}
+
+		// seek_request of p.requests[request_index]. PAIRED: requests 2r and 2r + 1 are the two halves of pair r (additive or blend), sharing
+		// the per request policies of pair r.
+		template<bool DB = false, class RS = ReqState, bool PAIRED = false>
+		__device__ __forceinline__ void seek_transform(const DecodeParams& p, uint32_t request_index, RS& rs)
+		{
+			seek_request<DB>(p, p.requests[request_index], PAIRED ? request_index >> 1 : request_index, rs);
 		}
 
 		// ---------------------------------------------------------------------------------------------------

@@ -35,6 +35,19 @@ namespace aclb200
 
 	namespace
 	{
+		// The layered decode keeps one slot per request beside the request states. op: the layer's ACLB200_LAYER_*, k_layer_base for the
+		// first layer of its stack that is not OFF, k_layer_unknown for an op above ACLB200_LAYER_ADDITIVE; weight: its blend weight.
+		// stack_base of slot i: the block-local request whose row holds stack i's running pose, k_no_base when stack i writes nothing.
+		// num_stacks of slot 0: the stacks of the block (read from here after the decode, so that no register holds it through the fold).
+		struct alignas(16) LayerSlot
+		{
+			uint32_t op;
+			float    weight;
+			uint32_t stack_base;
+			uint32_t num_stacks;
+		};
+		constexpr uint32_t k_layer_base = 3, k_layer_unknown = 4, k_no_base = 0xFFFFFFFFu;
+
 		// ---------------------------------------------------------------------------------------------------
 		// kernels
 		// ---------------------------------------------------------------------------------------------------
@@ -52,14 +65,19 @@ namespace aclb200
 		//             blend (aclb200_decompress_tracks_blend): from and to half, both full poses; row 2r becomes rtm::qvv_lerp(from, to, weight).
 		//             The object kind k_object_skinning (the _skinning entry points) is a run-time value like the other kinds: the matrix walk,
 		//             then the skinning step of object_space.cuh on the whole pose.
+		//             k_compose_layers (aclb200_decompress_tracks_layered): requests r L .. r L + L - 1 are the layers of stack r (L = p.num_layers
+		//             at run time, whole stacks per block), read as 16 byte aclb200_layer records. An OFF layer is not sought. Phase 4c folds the
+		//             later layers into the base row (the first layer that is not OFF) with the pair modes' blend_row / apply_additive_row;
+		//             phases 4b and 5 take the base row.
 		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
 			constexpr bool PAIRED = COMPOSE == k_compose_additive || COMPOSE == k_compose_blend;
+			constexpr bool LAYERED = COMPOSE == k_compose_layers;
 			static_assert(COMPOSE == k_compose_local || OUT_STAGED, "the composed decodes work on poses assembled in shared memory");
 			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
-			// dynamic shared memory: RS[requests_per_block] | key frame windows | pose staging
+			// dynamic shared memory: RS[requests_per_block] (LAYERED: then LayerSlot[requests_per_block]) | key frame windows | pose staging
 			extern __shared__ __align__(16) uint8_t s_dynamic[];
 			__shared__ __align__(8) uint64_t s_barrier;
 			RS* s_req = reinterpret_cast<RS*>(s_dynamic);
@@ -69,6 +87,13 @@ namespace aclb200
 
 			const uint32_t first_request = blockIdx.x * p.requests_per_block;
 			const uint32_t num_requests = min(p.requests_per_block, p.num_requests - first_request);
+			// LAYERED: what each layer does, and the block's stacks (requests_per_block and num_requests are multiples of L; recomputed or
+			// read back where they are used rather than kept live through the decode)
+			LayerSlot* s_layer = reinterpret_cast<LayerSlot*>(s_dynamic + size_t(p.requests_per_block) * sizeof(RS));
+			auto num_stacks = [&]() { return s_layer[0].num_stacks; };
+			auto first_stack = [&]() { return blockIdx.x * fast_div(p.requests_per_block, p.magic_layers); };
+			if (LAYERED && threadIdx.x == 0)
+				s_layer[0].num_stacks = fast_div(num_requests, p.magic_layers);
 
 			if (STAGED)
 			{
@@ -81,7 +106,23 @@ namespace aclb200
 			if (threadIdx.x < num_requests)
 			{
 				RS rs;
-				seek_transform<DB, RS, PAIRED>(p, first_request + threadIdx.x, rs);
+				if constexpr (LAYERED)
+				{
+					// an OFF layer (or an unknown op) never reaches the clip table; an ADDITIVE layer above the base takes the writer defaults
+					const aclb200_layer* stack_layers = reinterpret_cast<const aclb200_layer*>(p.requests) + first_request;
+					const uint32_t stack = fast_div(threadIdx.x, p.magic_layers);
+					const aclb200_layer layer = stack_layers[threadIdx.x];
+					bool base = layer.op == ACLB200_LAYER_BLEND || layer.op == ACLB200_LAYER_ADDITIVE;
+					for (uint32_t below = stack * p.num_layers; below < threadIdx.x; ++below)
+						base = base && __ldg(&stack_layers[below].op) == ACLB200_LAYER_OFF;
+					s_layer[threadIdx.x].op = layer.op > ACLB200_LAYER_ADDITIVE ? k_layer_unknown : (base ? k_layer_base : layer.op);
+					s_layer[threadIdx.x].weight = layer.weight;
+					rs.num_tracks = 0;
+					if (layer.op == ACLB200_LAYER_BLEND || layer.op == ACLB200_LAYER_ADDITIVE)
+						seek_request<DB>(p, layer.pose, first_stack() + stack, rs);
+				}
+				else
+					seek_transform<DB, RS, PAIRED>(p, first_request + threadIdx.x, rs);
 				rs.out = p.out + uint64_t(first_request + threadIdx.x) * p.pose_stride;
 				if (STAGED)
 				{
@@ -108,6 +149,28 @@ namespace aclb200
 			}
 			__syncthreads();
 
+			// ---- LAYERED: one thread per stack finds its base layer, or that the stack writes nothing (read after phase 4c's barrier) ----
+			if constexpr (LAYERED)
+			{
+				if (threadIdx.x < num_stacks())
+				{
+					uint32_t base = k_no_base;
+					bool valid = true;
+					for (uint32_t layer = threadIdx.x * p.num_layers; layer < (threadIdx.x + 1) * p.num_layers; ++layer)
+					{
+						const uint32_t op = s_layer[layer].op;
+						if (op == ACLB200_LAYER_OFF)
+							continue;
+						const uint32_t tracks = s_req[layer].num_tracks;
+						if (op == k_layer_unknown || tracks == 0 || (base != k_no_base && tracks != s_req[base].num_tracks))
+							valid = false;
+						if (base == k_no_base)
+							base = layer;
+					}
+					s_layer[threadIdx.x].stack_base = valid ? base : k_no_base;
+				}
+			}
+
 			// ---- phase 2: constant and default sub-tracks, one thread per (request, bone) ----
 			{
 				const uint32_t num_slots = num_requests * p.max_tracks;
@@ -121,7 +184,7 @@ namespace aclb200
 					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
 					uint8_t* pose = OUT_STAGED ? s_out + size_t(local_request) * p.smem_pose_bytes : rs.out;
 					constant_sub_tracks<NORM, false>(p, rs, bone, desc, pose + size_t(bone) * p.bone_stride,
-						COMPOSE == k_compose_additive && (local_request & 1u) != 0);
+						(COMPOSE == k_compose_additive && (local_request & 1u) != 0) || (LAYERED && s_layer[local_request].op == ACLB200_LAYER_ADDITIVE));
 				}
 			}
 
@@ -224,17 +287,63 @@ namespace aclb200
 				}
 			}
 
+			// ---- phase 4c, layers: one thread per (stack, bone) folds the layers above the base into the base row, in place and in layer order:
+			// BLEND lerps towards the layer's row, ADDITIVE applies the layer's row to the running one, OFF is passed over; stacks that write
+			// nothing are left alone ----
+			if constexpr (LAYERED)
+			{
+				__syncthreads();
+				const uint32_t num_slots = num_stacks() * p.max_tracks;
+				for (uint32_t slot = threadIdx.x; slot < num_slots; slot += k_threads_per_block)
+				{
+					const uint32_t stack = fast_div(slot, p.magic_tracks);
+					const uint32_t bone = slot - stack * p.max_tracks;
+					const uint32_t base = s_layer[stack].stack_base;
+					if (base == k_no_base || bone >= s_req[base].num_tracks)
+						continue;
+					uint8_t* row = s_out + size_t(base) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
+					for (uint32_t layer = base + 1; layer < (stack + 1) * p.num_layers; ++layer)
+					{
+						const uint32_t op = s_layer[layer].op;
+						const uint8_t* layer_row = s_out + size_t(layer) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
+						if (op == ACLB200_LAYER_BLEND)
+							obj::blend_row(row, row, layer_row, s_layer[layer].weight, p.layout == ACLB200_LAYOUT_QVV40);
+						else if (op == ACLB200_LAYER_ADDITIVE)
+						{
+							uint32_t format = p.additive_format;
+							if (p.clip_additive_formats != nullptr)
+							{
+								format = __ldg(p.clip_additive_formats + s_req[layer].clip);
+								format = format <= ACLB200_ADDITIVE_ADDITIVE1 ? format : ACLB200_ADDITIVE_NONE;		// apply_additive_to_base's `default:`
+							}
+							// (a flag is rare: reported where it is met, so that no accumulator stays live through the fold)
+							const uint32_t flags = obj::apply_additive_row(row, row, layer_row, format, p.layout == ACLB200_LAYOUT_QVV40);
+							if (flags != 0 && p.object_flags != nullptr)
+								atomicOr(p.object_flags, flags);
+						}
+					}
+				}
+			}
+
 			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (PAIRED: the
 			// combined row of each pair, when parents are given) ----
 			if constexpr (COMPOSE != k_compose_local)
 			{
-				if (!PAIRED || p.parent_indices != nullptr)
+				if ((!PAIRED && !LAYERED) || p.parent_indices != nullptr)
 				{
 					__syncthreads();
 					uint32_t flags = 0;
 					constexpr uint32_t step = PAIRED ? 2u : 1u;
-					for (uint32_t local_request = (threadIdx.x >> 5) * step; local_request < num_requests; local_request += (k_threads_per_block / 32) * step)
+					const uint32_t num_items = LAYERED ? num_stacks() : num_requests;
+					for (uint32_t item = (threadIdx.x >> 5) * step; item < num_items; item += (k_threads_per_block / 32) * step)
 					{
+						uint32_t local_request = item;
+						if constexpr (LAYERED)
+						{
+							local_request = s_layer[item].stack_base;
+							if (local_request == k_no_base)
+								continue;
+						}
 						const RS& rs = s_req[local_request];
 						if (rs.num_tracks == 0 || (PAIRED && s_req[local_request + 1].num_tracks != rs.num_tracks))
 							continue;
@@ -256,13 +365,19 @@ namespace aclb200
 			{
 				__syncthreads();
 				const uint32_t chunks_per_pose = p.smem_pose_bytes >> 4;
-				const uint32_t num_poses = PAIRED ? num_requests >> 1 : num_requests;
-				const uint32_t first_pose = PAIRED ? first_request >> 1 : first_request;
+				const uint32_t num_poses = PAIRED ? num_requests >> 1 : (LAYERED ? num_stacks() : num_requests);
+				const uint32_t first_pose = PAIRED ? first_request >> 1 : (LAYERED ? first_stack() : first_request);
 				const uint32_t num_chunks = num_poses * chunks_per_pose;
 				for (uint32_t slot = threadIdx.x; slot < num_chunks; slot += k_threads_per_block)
 				{
 					const uint32_t local_pose = fast_div(slot, p.magic_chunks);
-					const uint32_t local_request = PAIRED ? local_pose * 2 : local_pose;
+					uint32_t local_request = PAIRED ? local_pose * 2 : local_pose;
+					if constexpr (LAYERED)
+					{
+						local_request = s_layer[local_pose].stack_base;
+						if (local_request == k_no_base)
+							continue;
+					}
 					const uint32_t byte = (slot - local_pose * chunks_per_pose) << 4;
 					uint32_t row_bytes = s_req[local_request].num_tracks * p.bone_stride;
 					if (PAIRED && s_req[local_request + 1].num_tracks != s_req[local_request].num_tracks)
@@ -936,13 +1051,15 @@ namespace aclb200
 	// requests_per_block, the division magics and the shared memory carve-up of a launch
 	// compose != local: the composed decodes need every pose in shared memory, so a pose that does not fit gives up key frame staging
 	// instead (params.smem_bytes then tells the caller whether one request fits at all)
-	// additive, blend: requests_per_block stays even, so that the two halves of a pair always share a block
+	// additive, blend: requests_per_block stays even, so that the two halves of a pair always share a block; layers: a multiple of
+	// params.num_layers, so that a stack never spans two blocks (and each request carries a LayerSlot beside its state)
 	void plan_launch(DecodeParams& params, uint32_t max_key_frame_bytes, int max_dynamic_smem, bool allow_output_staging, bool database,
 		uint32_t compose)
 	{
 		const bool force_output_staging = compose != k_compose_local;
 		const bool pairs = compose == k_compose_additive || compose == k_compose_blend;
-		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
+		const bool layers = compose == k_compose_layers;
+		const uint32_t state_bytes = (database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState))) + (layers ? uint32_t(sizeof(LayerSlot)) : 0u);
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);
 		// ~28 KB of shared memory per block keeps 8 blocks resident per SM
@@ -955,9 +1072,8 @@ namespace aclb200
 		uint32_t requests_per_block = k_target_items_per_block / max_tracks;
 		if (requests_per_block < 1) requests_per_block = 1;
 		if (requests_per_block > k_max_requests_per_block) requests_per_block = k_max_requests_per_block;
-		const uint32_t step = pairs ? 2u : 1u;
-		if (pairs)
-			requests_per_block = requests_per_block < 2 ? 2u : (requests_per_block & ~1u);
+		const uint32_t step = layers ? params.num_layers : (pairs ? 2u : 1u);
+		requests_per_block = requests_per_block < step ? step : requests_per_block - requests_per_block % step;
 
 		auto bytes_needed = [&](uint32_t requests) { return requests * (state_bytes + 2 * stage_bytes + pose_bytes); };
 		while (requests_per_block > step && bytes_needed(requests_per_block) > block_budget)
@@ -978,6 +1094,7 @@ namespace aclb200
 		params.magic_rot = division_magic(params.max_animated[0]);
 		params.magic_vec = division_magic(params.max_animated[1] + params.max_animated[2]);
 		params.magic_chunks = division_magic(pose_bytes >> 4);
+		params.magic_layers = division_magic(params.num_layers);
 		params.out_vector16 = ((uint64_t(reinterpret_cast<uintptr_t>(params.out)) | params.pose_stride) & 15) == 0 ? 1u : 0u;
 	}
 

@@ -446,6 +446,20 @@ namespace acl_b200
 			m_device->check(aclb200_blend_poses(m_device->get(), d_from_poses, d_to_poses, d_out, num_poses, num_tracks, pose_stride_bytes, weight,
 				d_weights, stream), "aclb200_blend_poses");
 		}
+		// Up to eight layers per pose in one launch (aclb200_decompress_tracks_layered): pose r owns d_layers[r * num_layers + i]; the first
+		// layer that is not ACLB200_LAYER_OFF is the base, decoded as decompress_tracks decodes it, and each later layer is folded in, in
+		// order: BLEND = rtm::qvv_lerp(running, layer, weight), ADDITIVE = acl::apply_additive_to_base(format, running, layer) with the layer
+		// decoded with the track_writer defaults, OFF = skipped unread. Format: d_clip_additive_formats[layer clip] (nullptr: additive_format).
+		// With parents the running pose leaves in object space as object_kind rows (the base clip's skeleton), else as local rows in
+		// options.output_layout.
+		void decompress_tracks_layered(const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options& options,
+			uint32_t additive_format, const uint8_t* d_clip_additive_formats, void* d_out, const uint32_t* d_parent_indices = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr,
+			void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_layered(m_device->get(), m_clipset, d_layers, num_poses, num_layers, &options, additive_format,
+				d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_layered");
+		}
 		// Skinning rows: the ACLB200_OBJECT_MATRIX3X4F walk, then rtm::matrix_mul(inverse_bind, object) per bone, stored as three float4 rows,
 		// row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]). d_inverse_bind holds 12 floats per skeleton entry, 16 byte aligned, in
 		// parallel with d_parent_indices (aclb200_decompress_tracks_skinning and its additive, blend and standalone forms)
@@ -470,6 +484,14 @@ namespace acl_b200
 		{
 			m_device->check(aclb200_decompress_tracks_blend_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, weight, d_weights,
 				d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_blend_skinning");
+		}
+		void decompress_tracks_layered_skinning(const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options& options,
+			uint32_t additive_format, const uint8_t* d_clip_additive_formats, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+			const float* d_inverse_bind, void* d_out, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_layered_skinning(m_device->get(), m_clipset, d_layers, num_poses, num_layers, &options,
+				additive_format, d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream),
+				"aclb200_decompress_tracks_layered_skinning");
 		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,

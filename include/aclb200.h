@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 9
+#define ACLB200_VERSION_MINOR 10
 
 typedef enum aclb200_status
 {
@@ -533,6 +533,62 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_additive_skinning(aclb200_c
 ACLB200_API aclb200_status aclb200_decompress_tracks_blend_skinning(aclb200_context* context, const aclb200_clipset* clipset,
 	const aclb200_blend_request* d_requests, uint32_t num_requests, const aclb200_options* options,
 	float weight, const float* d_weights,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* What a layer does to the running pose of its stack (aclb200_decompress_tracks_layered) */
+enum { ACLB200_LAYER_OFF = 0, ACLB200_LAYER_BLEND = 1, ACLB200_LAYER_ADDITIVE = 2 };
+
+/* One layer of a layered pose: a clip of the clip set at its own sample time, and what it does to the poses below it */
+typedef struct aclb200_layer
+{
+	aclb200_request pose;			/* this layer's clip and sample time */
+	uint32_t op;					/* ACLB200_LAYER_* */
+	float    weight;				/* BLEND: the rtm::qvv_lerp weight, used as given (no clamp); ignored otherwise */
+} aclb200_layer;
+
+/* A pose graph of up to eight clips per pose in one kernel: every layer is decoded, and the layers are folded into the running pose in
+ * index order in shared memory; only the result leaves. Pose r owns the layers d_layers[r * num_layers + i], 1 <= num_layers <= 8:
+ *   base           the first layer whose op is not OFF, decoded exactly as aclb200_decompress_tracks decodes its request under `options`
+ *                  (its op and weight are ignored). The running pose starts as the base.
+ *   later layers   in index order:
+ *                    OFF       not sought, not decoded, not read (its clip and time may be anything, no key frame traffic): stacks of
+ *                              different depths share one launch
+ *                    BLEND     decoded as a full pose (as either half of aclb200_decompress_tracks_blend), then
+ *                              running = rtm::qvv_lerp(running, layer, weight), computed as aclb200_decompress_tracks_blend computes it
+ *                    ADDITIVE  decoded with the acl::track_writer defaults (as the additive half of aclb200_decompress_tracks_additive),
+ *                              then running = acl::apply_additive_to_base(format, running, layer), format = d_clip_additive_formats[the
+ *                              layer's clip] (a byte above 3 reads as none) when that pointer is not NULL, else additive_format
+ *   policies       d_request_policies[r] (options) applies to every layer of pose r
+ *   d_out          d_parent_indices == NULL: the running pose in options->output_layout (QVV48 or QVV40) at d_out + r * pose_stride
+ *                  (options->pose_stride_bytes, 0 = max_tracks * bone size). d_parent_indices given: the hierarchy walk of
+ *                  aclb200_decompress_tracks_object_space with the skeleton of the BASE layer's clip c (d_parent_indices +
+ *                  d_skeleton_offsets[c], d_skeleton_offsets NULL: 0), object_kind rows (QVV48 only).
+ *                  Pose r writes nothing when every layer is OFF, when a layer that is not OFF names an invalid clip or a clip whose track
+ *                  count differs from the base's, or when any layer's op is above 2. No byte past the base clip's num_tracks bones is written.
+ *   d_out_flags    device uint32, optional: cleared, then ACLB200_ERROR_FLAG_NEGATIVE_SCALE (a relative layer took qvv_mul's matrix branch,
+ *                  or the walk did) and ACLB200_ERROR_FLAG_INVALID_SKELETON OR-ed in
+ * Blend-space weights: the stack [clip 0 as base, clip 1 BLEND w_1, ..., clip n BLEND w_n] gives the normalised blend
+ * sum_i a_i clip_i (a_0 + ... + a_n = 1) of the lerps' translations and scales with the step weights
+ *     w_i = a_i / (a_0 + a_1 + ... + a_i)
+ * (each step's lerp keeps the ratios of the clips before it); additive layers then go on top.
+ * Every operation is IEEE and unfused; ACLB200_MATH_FAST is accepted and runs the exact decode.
+ * Refused, writing nothing and leaving *d_out_flags untouched: ACLB200_ERR_INVALID_ARGUMENT for num_layers 0 or above 8, num_poses *
+ * num_layers above 2^32 - 1, skip masks or a `skipped` default mode, additive_format > 3, a scalar clip set, an output that breaks the
+ * alignment rules of aclb200_decompress_tracks, and with parents an unknown object_kind or QVV40. ACLB200_ERR_UNSUPPORTED when
+ * num_layers poses of the widest clip do not fit in one block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_layered(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The skinning rows of the layered pose: aclb200_decompress_tracks_layered's running pose through the matrix walk and the skinning step
+ * of aclb200_decompress_tracks_skinning, with the base layer's skeleton and inverse binds (d_inverse_bind + 12 * d_skeleton_offsets[base
+ * clip]). Refusals as aclb200_decompress_tracks_layered, plus NULL parents and NULL or misaligned inverse binds. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_layered_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
 

@@ -2,7 +2,7 @@
 chained playback through the pipeline kernel (groups, tail crossing, base row reuse), ragged random requests, per track rounding,
 skipped defaults (plain kernels), decompress_track, the object space decode (both kinds, a skeleton per clip), the additive decode (local and
 object space, per clip formats) and aclb200_apply_additive_to_base, the blend decode (local and object space, a weight per pair) and
-aclb200_blend_poses, the chained scalar kernel."""
+aclb200_blend_poses, the skinning decodes, the layered decode (local, object space and skinning rows), the chained scalar kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -139,6 +139,30 @@ ctx.decompress_tracks(one, torch.from_numpy(ab.make_requests(np.zeros(64), np.li
 ctx.local_to_skinning(local, local, 64, one.max_tracks, d_parents, d_inverse)
 torch.cuda.synchronize()
 one.release()
+# layered decode: the layers instances (three layer stacks of one clip each: base, BLEND, ADDITIVE with the per clip formats, the middle
+# layer OFF on every other stack), local, object space and skinning rows
+from tests import layers_cases
+stacks = [[(c, float(pair_time[i, 0]), layers_cases.BLEND, 0.0),
+           (c, float(pair_time[i, 1]), layers_cases.BLEND if i % 2 else layers_cases.OFF, float(blend_weights[i])),
+           (c, float(pair_time[i, 0]) * 0.5, layers_cases.ADDITIVE, 0.0)] for i, c in enumerate(pair_clip)]
+stack_values = np.array(stacks, np.float64)
+d_layers = torch.from_numpy(ab.make_layers(stack_values[..., 0].astype(np.uint32), stack_values[..., 1], stack_values[..., 2].astype(np.uint32),
+                                           stack_values[..., 3]).reshape(-1).view(np.uint8)).cuda()
+for parents in (None, d_parents):
+    out = torch.zeros((len(stacks), cs.max_tracks, 12), dtype=torch.float32, device="cuda")
+    ctx.decompress_tracks_layered(cs, d_layers, len(stacks), 3, ab.Options(), out, d_clip_additive_formats=d_formats, d_parent_indices=parents,
+                                  d_skeleton_offsets=d_offsets)
+    torch.cuda.synchronize()
+    got = out.cpu().numpy()
+    for i in range(0, len(stacks), 5):
+        c = pair_clip[i]
+        want = layers_cases.port_local(port, blend, blobs, stacks[i], settings, writer, 0, 2, clip_formats=np.arange(len(names)) % 5)
+        if parents is not None:
+            want = port.local_to_object_space(want, trees[c], port.NORMALIZE_IEEE)
+        bad += not clips.bit_equal(got[i, :counts[c]][:, L], want[:, L])
+ctx.decompress_tracks_layered_skinning(cs, d_layers, len(stacks), 3, ab.Options(), d_parents, d_inverse, out, d_clip_additive_formats=d_formats,
+                                       d_skeleton_offsets=d_offsets)
+torch.cuda.synchronize()
 # scalar clips
 for name in ("float1", "float3", "vector4", "float1_c4_small"):
     blob = clips.load_blob(name); spec = clips.SCALAR_SPECS[name]
