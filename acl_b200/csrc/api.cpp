@@ -86,6 +86,14 @@ namespace aclb200
 				if ((params.pose_stride % alignment) != 0 || (reinterpret_cast<uintptr_t>(d_out) % alignment) != 0)
 					return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "the output pointer and pose_stride_bytes must keep bones 16 (QVV48) / 8 (QVV40) byte aligned");
 			}
+			else
+			{
+				// the scalar kernels store each component with one 4 byte store: a misaligned row would fault on the device
+				const uint64_t misaligned = reinterpret_cast<uintptr_t>(d_out) | (single_track ? 0u : params.pose_stride);
+				if ((misaligned % 4) != 0)
+					return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, single_track ? "the output pointer must be 4 byte aligned"
+						: "the output pointer and pose_stride_bytes must be multiples of 4");
+			}
 			params.rounding_policy = options->rounding_policy;
 			params.looping_policy = options->looping_policy;
 			params.normalization = options->normalization;
@@ -763,9 +771,13 @@ extern "C"
 			if (first == last)
 				continue;
 			uint8_t* d_chunk = d_out + size_t(first) * pose_stride;
+			// a chunk's requests start at `first`: so do their policy pairs
+			aclb200_options chunk_options = *options;
+			if (chunk_options.d_request_policies != nullptr)
+				chunk_options.d_request_policies += size_t(first) * 2;
 			const aclb200_status status = is_transform
-				? aclb200_decompress_tracks(context, clipset, d_requests + first, last - first, options, d_chunk, stream)
-				: aclb200_scalar_decompress_tracks(context, clipset, d_requests + first, last - first, options, d_chunk, stream);
+				? aclb200_decompress_tracks(context, clipset, d_requests + first, last - first, &chunk_options, d_chunk, stream)
+				: aclb200_scalar_decompress_tracks(context, clipset, d_requests + first, last - first, &chunk_options, d_chunk, stream);
 			if (status != ACLB200_OK)
 			{
 				cudaStreamSynchronize(stream);
