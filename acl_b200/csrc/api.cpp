@@ -25,19 +25,26 @@ namespace aclb200
 				|| options.default_scale_mode == ACLB200_DEFAULT_SKIPPED || (options.skip_mask & 7u) != 0 || options.d_skip_track_mask != nullptr;
 		}
 
-		// the C entry point of each compose mode, for messages
-		const char* const k_compose_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_object_space", "decompress_tracks_additive",
-			"decompress_tracks_blend", "decompress_tracks_layered" };
-		const char* const k_skinning_entry[k_compose_count] = { "decompress_tracks", "decompress_tracks_skinning", "decompress_tracks_additive_skinning",
-			"decompress_tracks_blend_skinning", "decompress_tracks_layered_skinning" };
-		// what a composed decode that does not fit one block is refused with
-		const char* const k_unfit_message[k_compose_count] = { "", ": one pose does not fit in a block's shared memory",
-			": the two poses of a pair do not fit in a block's shared memory", ": the two poses of a pair do not fit in a block's shared memory",
-			": the poses of a layer stack do not fit in a block's shared memory" };
+		// What a composed entry point launches: pose r is the launch's requests r L .. r L + L - 1, combined by the compose mode
+		struct Composed
+		{
+			const char* entry;						// the C entry point, for messages
+			const char* unfit;						// the refusal of a pose whose requests do not fit one block's shared memory
+			uint32_t compose;						// k_compose_*
+			uint32_t num_layers;					// L: 1 (object), 2 (additive, blend) or the layered decode's num_layers
+			float weight;							// blend: the weight of every pair when d_weights is NULL
+			const float* d_weights;					// blend: [pairs] the weight of each pair, or NULL
+			uint32_t additive_format;				// additive, layers: the format when d_clip_additive_formats is NULL
+			const uint8_t* d_clip_additive_formats;	// additive, layers: [num_clips] the format of each clip, or NULL
+		};
+		const char* const k_pose_unfit = ": one pose does not fit in a block's shared memory";
+		const char* const k_pair_unfit = ": the two poses of a pair do not fit in a block's shared memory";
+		const char* const k_layers_unfit = ": the poses of a layer stack do not fit in a block's shared memory";
 
+		// composed: the description of a composed decode, nullptr for the plain decode
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
 			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			uint32_t compose = k_compose_local, uint32_t num_layers = 1)
+			const Composed* composed = nullptr)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
@@ -126,11 +133,12 @@ namespace aclb200
 				params.db_bulk[1] = clipset->database->d_bulk[1];
 			}
 			// an object transform needs every sub-track of its parents, apply_additive_to_base and qvv_lerp every sub-track of both poses
-			if (compose != k_compose_local && keeps_bytes)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(k_compose_entry[compose])
+			if (composed != nullptr && keeps_bytes)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(composed->entry)
 					+ ": the composed poses need every decoded sub-track (no skip masks, no `skipped` default mode)");
-			params.num_layers = num_layers;
-			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !keeps_bytes, database, compose);
+			params.num_layers = composed != nullptr ? composed->num_layers : 1u;
+			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !keeps_bytes, database,
+				composed != nullptr ? composed->compose : k_compose_local);
 			return ACLB200_OK;
 		}
 
@@ -141,20 +149,20 @@ namespace aclb200
 			return check_cuda(context, error, what);
 		}
 
-		// The composed decodes. Every refusal comes before the flags are cleared: a refused call writes nothing. d_inverse_bind is given by
-		// the skinning entry points only (they require parents), and makes the object kind k_object_skinning.
-		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
-			uint32_t num_requests, const aclb200_options* options, uint32_t compose, const uint32_t* d_parent_indices,
-			const uint32_t* d_skeleton_offsets, const float* d_inverse_bind, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream,
-			const std::function<void(DecodeParams&)>& set_pair_operands = nullptr, uint32_t num_layers = 1)
+		// The composed decodes: num_poses poses of composed.num_layers requests each at d_requests. Every refusal comes before the flags are
+		// cleared: a refused call writes nothing. d_inverse_bind is given by the skinning entry points only (they require parents), and
+		// makes the object kind k_object_skinning.
+		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const void* d_requests, uint32_t num_poses,
+			const aclb200_options* options, const Composed& composed, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+			const float* d_inverse_bind, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream)
 		{
-			const std::string entry = d_inverse_bind != nullptr ? k_skinning_entry[compose] : k_compose_entry[compose];
+			const std::string entry = composed.entry;
 			DecodeParams params;
-			const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params, compose,
-				num_layers);
+			const aclb200_status status = make_params(context, clipset, static_cast<const aclb200_request*>(d_requests), num_poses * composed.num_layers,
+				options, d_out, true, false, params, &composed);
 			if (status != ACLB200_OK)
 				return status;
-			// object space output: always in the object space decode (its entry point requires parents), with parents in the paired ones
+			// object space output: always in the object space decode (its entry point requires parents), with parents in the others
 			if (d_inverse_bind != nullptr)
 				object_kind = k_object_skinning;
 			else if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
@@ -163,22 +171,24 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
 			// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
 			if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + k_unfit_message[compose]);
-			if (num_requests == 0)
+				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + composed.unfit);
+			if (num_poses == 0)
 				return ACLB200_OK;
 			params.parent_indices = d_parent_indices;
 			params.skeleton_offsets = d_skeleton_offsets;
 			params.object_flags = d_out_flags;
 			params.object_kind = object_kind;
 			params.inverse_bind = d_inverse_bind;
-			if (set_pair_operands)
-				set_pair_operands(params);
+			params.blend_weight = composed.weight;
+			params.blend_weights = composed.d_weights;
+			params.additive_format = composed.additive_format;
+			params.clip_additive_formats = composed.d_clip_additive_formats;
 			cudaSetDevice(context->device);
 			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 			const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, entry.c_str());
 			if (cleared != ACLB200_OK)
 				return cleared;
-			return finish_launch(context, launch_transform_decompress_tracks(params, compose, params.db_tiers != nullptr, cuda_stream), entry.c_str());
+			return finish_launch(context, launch_transform_decompress_tracks(params, composed.compose, params.db_tiers != nullptr, cuda_stream), entry.c_str());
 		}
 	}
 
@@ -442,8 +452,9 @@ extern "C"
 	{
 		if (d_parent_indices == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: null parent index pointer");
-		return decompress_composed(context, clipset, d_requests, num_requests, options, k_compose_object, d_parent_indices, d_skeleton_offsets,
-			nullptr, object_kind, d_out, d_out_flags, stream);
+		const Composed composed = { "decompress_tracks_object_space", k_pose_unfit, k_compose_object, 1 };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
+			object_kind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -454,8 +465,9 @@ extern "C"
 		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_skinning");
 		if (status != ACLB200_OK)
 			return status;
-		return decompress_composed(context, clipset, d_requests, num_requests, options, k_compose_object, d_parent_indices, d_skeleton_offsets,
-			d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream);
+		const Composed composed = { "decompress_tracks_skinning", k_pose_unfit, k_compose_object, 1 };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
+			k_object_skinning, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
@@ -470,12 +482,10 @@ extern "C"
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: additive_format out of range");
 		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
 		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_additive,
-			d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
-			{
-				params.additive_format = additive_format;
-				params.clip_additive_formats = d_clip_additive_formats;
-			});
+		const Composed composed = { "decompress_tracks_additive", k_pair_unfit, k_compose_additive, 2, 0.0f, nullptr, additive_format,
+			d_clip_additive_formats };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
+			object_kind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -491,12 +501,10 @@ extern "C"
 		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_additive_skinning");
 		if (status != ACLB200_OK)
 			return status;
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_additive,
-			d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream, [&](DecodeParams& params)
-			{
-				params.additive_format = additive_format;
-				params.clip_additive_formats = d_clip_additive_formats;
-			});
+		const Composed composed = { "decompress_tracks_additive_skinning", k_pair_unfit, k_compose_additive, 2, 0.0f, nullptr, additive_format,
+			d_clip_additive_formats };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
+			k_object_skinning, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
@@ -536,12 +544,9 @@ extern "C"
 		// pair r is the two requests 2r (from) and 2r + 1 (to) of the plain decode, the layout of aclb200_additive_request
 		static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
 			"a blend request is two requests back to back");
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_blend,
-			d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
-			{
-				params.blend_weight = weight;
-				params.blend_weights = d_weights;
-			});
+		const Composed composed = { "decompress_tracks_blend", k_pair_unfit, k_compose_blend, 2, weight, d_weights };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
+			object_kind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_blend_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -555,12 +560,9 @@ extern "C"
 		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_blend_skinning");
 		if (status != ACLB200_OK)
 			return status;
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), 2 * num_requests, options, k_compose_blend,
-			d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream, [&](DecodeParams& params)
-			{
-				params.blend_weight = weight;
-				params.blend_weights = d_weights;
-			});
+		const Composed composed = { "decompress_tracks_blend_skinning", k_pair_unfit, k_compose_blend, 2, weight, d_weights };
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
+			k_object_skinning, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered(aclb200_context* context, const aclb200_clipset* clipset,
@@ -574,12 +576,10 @@ extern "C"
 			return status;
 		// stack r is the requests r L .. r L + L - 1 of the launch, read as layer records by the kernel
 		static_assert(sizeof(aclb200_layer) == 16 && offsetof(aclb200_layer, pose) == 0, "a layer is a request, its op and its weight");
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_layers), num_poses * num_layers, options,
-			k_compose_layers, d_parent_indices, d_skeleton_offsets, nullptr, object_kind, d_out, d_out_flags, stream, [&](DecodeParams& params)
-			{
-				params.additive_format = additive_format;
-				params.clip_additive_formats = d_clip_additive_formats;
-			}, num_layers);
+		const Composed composed = { "decompress_tracks_layered", k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format,
+			d_clip_additive_formats };
+		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, nullptr, object_kind,
+			d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -593,13 +593,10 @@ extern "C"
 			status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_layered_skinning");
 		if (status != ACLB200_OK)
 			return status;
-		return decompress_composed(context, clipset, reinterpret_cast<const aclb200_request*>(d_layers), num_poses * num_layers, options,
-			k_compose_layers, d_parent_indices, d_skeleton_offsets, d_inverse_bind, k_object_skinning, d_out, d_out_flags, stream,
-			[&](DecodeParams& params)
-			{
-				params.additive_format = additive_format;
-				params.clip_additive_formats = d_clip_additive_formats;
-			}, num_layers);
+		const Composed composed = { "decompress_tracks_layered_skinning", k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format,
+			d_clip_additive_formats };
+		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
+			k_object_skinning, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

@@ -410,7 +410,8 @@ def test_wide_pose_limits(gpu):
 
 
 def test_refusals_write_nothing(gpu):
-    """Every refusal of the four entry points returns before the flags are cleared: neither the output nor the flags change."""
+    """Every refusal of the four entry points returns before the flags are cleared: neither the output nor the flags change. A launch that
+    would keep the caller's bytes (skip masks, a `skipped` default mode) is refused with a message that names the entry point called."""
     torch, ab, ctx = gpu["torch"], gpu["ab"], gpu["ctx"]
     clipset = ctx.upload([clips.load_blob("c1_30bones")])
     scalar = ctx.upload([clips.load_blob("float1")])
@@ -420,10 +421,11 @@ def test_refusals_write_nothing(gpu):
     inverse = _dev(gpu, np.concatenate([cases.random_affine(30, 1).reshape(-1), np.zeros(4, np.float32)]))
     aligned = inverse.data_ptr()
     skip_tracks = torch.zeros(30, dtype=torch.uint8, device="cuda")
+    keeps_bytes = "the composed poses need every decoded sub-track (no skip masks, no `skipped` default mode)"
     decode_refusals = [
-        dict(options=ab.Options(skip_mask=ab.SKIP_SCALE)),
-        dict(options=ab.Options(d_skip_track_mask=skip_tracks.data_ptr())),
-        dict(options=ab.Options(default_modes=(ab.DEFAULT_CONSTANT, ab.DEFAULT_SKIPPED, ab.DEFAULT_LEGACY))),
+        dict(options=ab.Options(skip_mask=ab.SKIP_SCALE), message=keeps_bytes),
+        dict(options=ab.Options(d_skip_track_mask=skip_tracks.data_ptr()), message=keeps_bytes),
+        dict(options=ab.Options(default_modes=(ab.DEFAULT_CONSTANT, ab.DEFAULT_SKIPPED, ab.DEFAULT_LEGACY)), message=keeps_bytes),
         dict(options=ab.Options(output_layout=ab.LAYOUT_QVV40)),
         dict(parents=0),
         dict(inverse=0),
@@ -431,9 +433,9 @@ def test_refusals_write_nothing(gpu):
         dict(clipset=scalar),
         dict(offset=8),
     ]
-    routes = [("plain", ctx.decompress_tracks_skinning, plain_requests, {}),
-              ("additive", ctx.decompress_tracks_additive_skinning, pair_requests, dict(additive_format=1)),
-              ("blend", ctx.decompress_tracks_blend_skinning, pair_requests, dict(weight=0.5))]
+    routes = [("decompress_tracks_skinning", ctx.decompress_tracks_skinning, plain_requests, {}),
+              ("decompress_tracks_additive_skinning", ctx.decompress_tracks_additive_skinning, pair_requests, dict(additive_format=1)),
+              ("decompress_tracks_blend_skinning", ctx.decompress_tracks_blend_skinning, pair_requests, dict(weight=0.5))]
     cases_ = [(route, case) for route in routes for case in decode_refusals]
     cases_.append((routes[1][:3] + (dict(additive_format=4),), {}))
     for (route, call, requests, extra), case in cases_:
@@ -443,6 +445,8 @@ def test_refusals_write_nothing(gpu):
             call(case.get("clipset", clipset), requests, 8, case.get("options", ab.Options()), case.get("parents", parents),
                  case.get("inverse", aligned), buffer.data_ptr() + case.get("offset", 0), d_out_flags=d_flags, **extra)
         assert error.value.status == 1, (route, case, extra)      # ACLB200_ERR_INVALID_ARGUMENT
+        if "message" in case:
+            assert str(error.value).endswith(f"{route}: {case['message']}"), (route, str(error.value))
         torch.cuda.synchronize()
         assert (buffer.cpu().numpy() == 0x5A).all(), (route, case)
         assert int(d_flags.item()) == 0x5A5A5A5A, (route, case)
