@@ -17,5 +17,5 @@ from .api import (  # noqa: F401
     OBJECT_QVVF, OBJECT_MATRIX3X4F,
     ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1, ADDITIVE_REQUEST_DTYPE, make_additive_requests,
     BLEND_REQUEST_DTYPE, make_blend_requests,
-    LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE, MAX_LAYERS, LAYER_DTYPE, make_layers,
+    LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE, LAYER_NO_MASK, MAX_LAYERS, LAYER_DTYPE, make_layers,
 )

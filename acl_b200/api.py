@@ -169,6 +169,10 @@ def _lib():
         l.aclb200_local_to_skinning.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, vp, vp]
         l.aclb200_decompress_tracks_layered.argtypes = [vp, vp, vp, u32, u32, C.POINTER(Options), u32, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_decompress_tracks_layered_skinning.argtypes = [vp, vp, vp, u32, u32, C.POINTER(Options), u32, vp, vp, vp, vp, vp, vp, vp]
+        l.aclb200_decompress_tracks_layered_masked.argtypes = [vp, vp, vp, vp, u32, u32, vp, u32, u32, C.POINTER(Options), u32, vp, vp, vp, u32,
+                                                               vp, vp, vp]
+        l.aclb200_decompress_tracks_layered_masked_skinning.argtypes = [vp, vp, vp, vp, u32, u32, vp, u32, u32, C.POINTER(Options), u32, vp, vp,
+                                                                        vp, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -199,6 +203,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_blend", "aclb200_blend_poses", "aclb200_decompress_tracks_skinning",
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
+        "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning",
     ]
 
 
@@ -242,6 +247,7 @@ def make_blend_requests(from_clips, from_times, to_clips, to_times) -> np.ndarra
 
 LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE = 0, 1, 2
 MAX_LAYERS = 8
+LAYER_NO_MASK = 0xFFFFFFFF      # the mask index of a layer without a bone mask (decompress_tracks_layered_masked)
 LAYER_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("op", np.uint32), ("weight", np.float32)])
 
 
@@ -482,6 +488,21 @@ class Context:
                                                              _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
                                                              _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
+    def decompress_tracks_layered_masked(self, clipset: ClipSet, d_layers, num_poses: int, num_layers: int, options: Options, d_out,
+                                         d_layer_masks=None, d_bone_masks=None, num_masks: int = 0, mask_stride: int = 0,
+                                         additive_format: int = 0, d_clip_additive_formats=None, d_parent_indices=None, kind: int = 0,
+                                         d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_layered with bone masks and weighted additive layers. d_layer_masks: uint32 [num_poses * num_layers] mask
+        index per layer (LAYER_NO_MASK: none; None: no layer has a mask); mask m is d_bone_masks[m * mask_stride + b] (float32, one per
+        bone of the base clip, mask_stride 0 = max_tracks). At bone b a layer's weight is weight * mask[b]; a mask of +-0 leaves the bone
+        untouched. BLEND = qvv_lerp(running, layer, w_b); ADDITIVE = apply_additive_to_base(format, running, layer) when w_b == 1, else
+        with qvv_lerp(writer defaults, layer, w_b) as the layer. ADDITIVE weights 1 and no masks give decompress_tracks_layered's bytes."""
+        self._check(_lib().aclb200_decompress_tracks_layered_masked(self._handle, clipset._handle, _device_ptr(d_layers), _device_ptr(d_layer_masks),
+                                                                    num_poses, num_layers, _device_ptr(d_bone_masks), num_masks, mask_stride,
+                                                                    C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
+                                                                    _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
+                                                                    _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as
     # three float4 rows, row c = (x_axis[c], y_axis[c], z_axis[c], w_axis[c]) of the skinning matrix: skinned[c] = dot(row c, (p, 1)). ----
@@ -522,6 +543,19 @@ class Context:
                                                                       _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
                                                                       _device_ptr(d_inverse_bind), _device_ptr(d_out), _device_ptr(d_out_flags),
                                                                       _stream_ptr(stream)))
+
+    def decompress_tracks_layered_masked_skinning(self, clipset: ClipSet, d_layers, num_poses: int, num_layers: int, options: Options,
+                                                  d_parent_indices, d_inverse_bind, d_out, d_layer_masks=None, d_bone_masks=None,
+                                                  num_masks: int = 0, mask_stride: int = 0, additive_format: int = 0,
+                                                  d_clip_additive_formats=None, d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_layered_masked's running poses as skinning rows, with the base clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_layered_masked_skinning(self._handle, clipset._handle, _device_ptr(d_layers),
+                                                                             _device_ptr(d_layer_masks), num_poses, num_layers,
+                                                                             _device_ptr(d_bone_masks), num_masks, mask_stride, C.byref(options),
+                                                                             additive_format, _device_ptr(d_clip_additive_formats),
+                                                                             _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                                             _device_ptr(d_inverse_bind), _device_ptr(d_out),
+                                                                             _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     def local_to_skinning(self, d_local_poses, d_out, num_poses: int, num_tracks: int, d_parent_indices, d_inverse_bind,
                           pose_stride_bytes: int = 0, d_out_flags=None, stream=None) -> None:

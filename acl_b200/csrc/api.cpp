@@ -36,6 +36,11 @@ namespace aclb200
 			const float* d_weights;					// blend: [pairs] the weight of each pair, or NULL
 			uint32_t additive_format;				// additive, layers: the format when d_clip_additive_formats is NULL
 			const uint8_t* d_clip_additive_formats;	// additive, layers: [num_clips] the format of each clip, or NULL
+			// layers_masked: the mask table (every field 0 in the other modes)
+			const uint32_t* d_layer_masks;			// [num_poses * num_layers] the mask index of each layer, or NULL
+			const float* d_bone_masks;				// [num_masks][mask_stride]
+			uint32_t num_masks;
+			uint32_t mask_stride;					// resolved by check_layer_masks (0 = max_tracks)
 		};
 		const char* const k_pose_unfit = ": one pose does not fit in a block's shared memory";
 		const char* const k_pair_unfit = ": the two poses of a pair do not fit in a block's shared memory";
@@ -183,6 +188,10 @@ namespace aclb200
 			params.blend_weights = composed.d_weights;
 			params.additive_format = composed.additive_format;
 			params.clip_additive_formats = composed.d_clip_additive_formats;
+			params.layer_masks = composed.d_layer_masks;
+			params.bone_masks = composed.d_bone_masks;
+			params.num_masks = composed.num_masks;
+			params.mask_stride = composed.mask_stride;
 			cudaSetDevice(context->device);
 			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 			const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, entry.c_str());
@@ -238,6 +247,33 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": additive_format out of range");
 			return ACLB200_OK;
 		}
+
+		// what the two masked layered decodes check of their own: the mask table, when a layer may name a mask; fills the Composed's mask
+		// fields (mask_stride 0 becomes max_tracks). A null clip set is left to make_params.
+		aclb200_status check_layer_masks(aclb200_context* context, const aclb200_clipset* clipset, const uint32_t* d_layer_masks,
+			const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const char* what, Composed& composed)
+		{
+			if (d_layer_masks == nullptr)
+				return ACLB200_OK;
+			if (d_bone_masks == nullptr || num_masks == 0)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": layer masks need d_bone_masks and num_masks >= 1");
+			if ((reinterpret_cast<uintptr_t>(d_bone_masks) % 4) != 0)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": d_bone_masks must be 4 byte aligned");
+			if (num_masks > k_max_layer_masks)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": num_masks is above 2^29 - 1");
+			const uint32_t max_tracks = clipset != nullptr ? clipset->info.max_tracks : 0u;
+			if (mask_stride == 0)
+				mask_stride = max_tracks;
+			if (mask_stride < max_tracks)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": mask_stride is below the clip set's max_tracks");
+			if (uint64_t(num_masks) * mask_stride > 0xFFFFFFFFu)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": num_masks * mask_stride is above 2^32 - 1");
+			composed.d_layer_masks = d_layer_masks;
+			composed.d_bone_masks = d_bone_masks;
+			composed.num_masks = num_masks;
+			composed.mask_stride = mask_stride;
+			return ACLB200_OK;
+		}
 	}
 }
 
@@ -247,7 +283,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.10 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.11 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -595,6 +631,44 @@ extern "C"
 			return status;
 		const Composed composed = { "decompress_tracks_layered_skinning", k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format,
 			d_clip_additive_formats };
+		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
+			k_object_skinning, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_tracks_layered_masked(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers,
+		const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		const char* what = "decompress_tracks_layered_masked";
+		Composed composed = { what, k_layers_unfit, k_compose_layers_masked, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
+		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
+		if (status == ACLB200_OK)
+			status = check_layer_masks(context, clipset, d_layer_masks, d_bone_masks, num_masks, mask_stride, what, composed);
+		if (status != ACLB200_OK)
+			return status;
+		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, nullptr, object_kind,
+			d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_tracks_layered_masked_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers,
+		const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options* options,
+		uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		const char* what = "decompress_tracks_layered_masked_skinning";
+		Composed composed = { what, k_layers_unfit, k_compose_layers_masked, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
+		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
+		if (status == ACLB200_OK)
+			status = check_layer_masks(context, clipset, d_layer_masks, d_bone_masks, num_masks, mask_stride, what, composed);
+		if (status == ACLB200_OK)
+			status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, what);
+		if (status != ACLB200_OK)
+			return status;
 		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
 			k_object_skinning, d_out, d_out_flags, stream);
 	}

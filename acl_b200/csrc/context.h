@@ -200,17 +200,28 @@ namespace aclb200
 		// the layers of output r (additive_format and clip_additive_formats as above)
 		uint32_t num_layers;						// L, 1..k_max_layers
 		uint32_t magic_layers;						// division_magic(L), for block-local indices
+		// the masked layered decode (aclb200_decompress_tracks_layered_masked, k_compose_layers_masked)
+		const uint32_t* layer_masks;				// [num_requests] the mask index of each layer (ACLB200_LAYER_NO_MASK: none), or nullptr
+		const float* bone_masks;					// [num_masks][mask_stride] one weight per bone of the base clip
+		uint32_t num_masks;							// at most k_max_layer_masks
+		uint32_t mask_stride;
 	};
 
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
-	// (aclb200_decompress_tracks_layered).
+	// (aclb200_decompress_tracks_layered). layers_masked: the layers mode with bone masks and weighted ADDITIVE layers
+	// (aclb200_decompress_tracks_layered_masked).
 	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_layers = 4,
-		k_compose_count = 5 };
+		k_compose_layers_masked = 5, k_compose_count = 6 };
 
 	// the deepest layer stack of aclb200_decompress_tracks_layered
 	constexpr uint32_t k_max_layers = 8;
+
+	// the most bone masks of one aclb200_decompress_tracks_layered_masked launch: a layer's slot keeps its mask index + 1 in the 29 bits
+	// above its op
+	constexpr uint32_t k_layer_op_bits = 3;
+	constexpr uint32_t k_max_layer_masks = (1u << (32 - k_layer_op_bits)) - 1;
 
 	// The object kind of the skinning decodes (after ACLB200_OBJECT_QVVF and ACLB200_OBJECT_MATRIX3X4F, never taken from a caller): the
 	// matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone, stored as the transposed rows a skinning shader reads

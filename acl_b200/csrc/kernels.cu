@@ -36,7 +36,9 @@ namespace aclb200
 	namespace
 	{
 		// The layered decode keeps one slot per request beside the request states. op: the layer's ACLB200_LAYER_*, k_layer_base for the
-		// first layer of its stack that is not OFF, k_layer_unknown for an op above ACLB200_LAYER_ADDITIVE; weight: its blend weight.
+		// first layer of its stack that is not OFF, k_layer_unknown for an op above ACLB200_LAYER_ADDITIVE (or, masked decode, a mask index
+		// at or above num_masks), in the low k_layer_op_bits; masked decode: above them the layer's mask index + 1 (0: no mask; only BLEND
+		// and ADDITIVE layers above the base carry one); weight: its weight.
 		// stack_base of slot i: the block-local request whose row holds stack i's running pose, k_no_base when stack i writes nothing.
 		// num_stacks of slot 0: the stacks of the block (read from here after the decode, so that no register holds it through the fold).
 		struct alignas(16) LayerSlot
@@ -46,7 +48,17 @@ namespace aclb200
 			uint32_t stack_base;
 			uint32_t num_stacks;
 		};
+		static_assert(sizeof(LayerSlot) == 16, "a layer slot is 16 bytes beside each request state");
 		constexpr uint32_t k_layer_base = 3, k_layer_unknown = 4, k_no_base = 0xFFFFFFFFu;
+		constexpr uint32_t k_layer_op_mask = (1u << k_layer_op_bits) - 1;
+
+		// The track_writer default pose as one pose row, [QVV40][scale one]: identity rotation, zero translation, scale 0 or 1 (the clip's
+		// k_clip_default_scale_one), QVV48 (rotation, translation + 0, scale + 0) and QVV40 (rotation, translation, scale) rows. It is the
+		// identity of every additive format: a weighted ADDITIVE layer lerps its row from it.
+		__device__ __align__(16) const float k_writer_default_rows[2][2][12] = {
+			{ { 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 0, 0 }, { 0, 0, 0, 1, 0, 0, 0, 0, 1, 1, 1, 0 } },
+			{ { 0, 0, 0, 1, 0, 0, 0, 0, 0, 0, 0, 0 }, { 0, 0, 0, 1, 0, 0, 0, 1, 1, 1, 0, 0 } },
+		};
 
 		// ---------------------------------------------------------------------------------------------------
 		// kernels
@@ -69,12 +81,18 @@ namespace aclb200
 		//             at run time, whole stacks per block), read as 16 byte aclb200_layer records. An OFF layer is not sought. Phase 4c folds the
 		//             later layers into the base row (the first layer that is not OFF) with the pair modes' blend_row / apply_additive_row;
 		//             phases 4b and 5 take the base row.
+		//             k_compose_layers_masked (aclb200_decompress_tracks_layered_masked): the layered mode where each layer may carry a bone
+		//             mask (its weight times mask[bone], skipped where the mask is +-0) and ADDITIVE layers take their weight. A mode of its
+		//             own rather than a run-time switch of k_compose_layers: the switch made the unmasked fold 1.4 % slower on C2.
 		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
 		{
 			constexpr bool PAIRED = COMPOSE == k_compose_additive || COMPOSE == k_compose_blend;
-			constexpr bool LAYERED = COMPOSE == k_compose_layers;
+			constexpr bool MASKED = COMPOSE == k_compose_layers_masked;
+			constexpr bool LAYERED = COMPOSE == k_compose_layers || MASKED;
+			// MASKED: a layer slot's op carries the layer's mask index above its low k_layer_op_bits
+			auto slot_op = [](uint32_t slot) { return MASKED ? slot & k_layer_op_mask : slot; };
 			static_assert(COMPOSE == k_compose_local || OUT_STAGED, "the composed decodes work on poses assembled in shared memory");
 			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
 			// dynamic shared memory: RS[requests_per_block] (LAYERED: then LayerSlot[requests_per_block]) | key frame windows | pose staging
@@ -115,7 +133,15 @@ namespace aclb200
 					bool base = layer.op == ACLB200_LAYER_BLEND || layer.op == ACLB200_LAYER_ADDITIVE;
 					for (uint32_t below = stack * p.num_layers; below < threadIdx.x; ++below)
 						base = base && __ldg(&stack_layers[below].op) == ACLB200_LAYER_OFF;
-					s_layer[threadIdx.x].op = layer.op > ACLB200_LAYER_ADDITIVE ? k_layer_unknown : (base ? k_layer_base : layer.op);
+					uint32_t op = layer.op > ACLB200_LAYER_ADDITIVE ? k_layer_unknown : (base ? k_layer_base : layer.op);
+					// MASKED: the mask index of a BLEND or ADDITIVE layer above the base, read beside its record
+					if (MASKED && p.layer_masks != nullptr && (op == ACLB200_LAYER_BLEND || op == ACLB200_LAYER_ADDITIVE))
+					{
+						const uint32_t mask = __ldg(p.layer_masks + first_request + threadIdx.x);
+						if (mask != ACLB200_LAYER_NO_MASK)
+							op = mask < p.num_masks ? op | ((mask + 1) << k_layer_op_bits) : k_layer_unknown;
+					}
+					s_layer[threadIdx.x].op = op;
 					s_layer[threadIdx.x].weight = layer.weight;
 					rs.num_tracks = 0;
 					if (layer.op == ACLB200_LAYER_BLEND || layer.op == ACLB200_LAYER_ADDITIVE)
@@ -158,7 +184,7 @@ namespace aclb200
 					bool valid = true;
 					for (uint32_t layer = threadIdx.x * p.num_layers; layer < (threadIdx.x + 1) * p.num_layers; ++layer)
 					{
-						const uint32_t op = s_layer[layer].op;
+						const uint32_t op = slot_op(s_layer[layer].op);
 						if (op == ACLB200_LAYER_OFF)
 							continue;
 						const uint32_t tracks = s_req[layer].num_tracks;
@@ -184,7 +210,7 @@ namespace aclb200
 					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
 					uint8_t* pose = OUT_STAGED ? s_out + size_t(local_request) * p.smem_pose_bytes : rs.out;
 					constant_sub_tracks<NORM, false>(p, rs, bone, desc, pose + size_t(bone) * p.bone_stride,
-						(COMPOSE == k_compose_additive && (local_request & 1u) != 0) || (LAYERED && s_layer[local_request].op == ACLB200_LAYER_ADDITIVE));
+						(COMPOSE == k_compose_additive && (local_request & 1u) != 0) || (LAYERED && slot_op(s_layer[local_request].op) == ACLB200_LAYER_ADDITIVE));
 				}
 			}
 
@@ -289,7 +315,7 @@ namespace aclb200
 
 			// ---- phase 4c, layers: one thread per (stack, bone) folds the layers above the base into the base row, in place and in layer order:
 			// BLEND lerps towards the layer's row, ADDITIVE applies the layer's row to the running one, OFF is passed over; stacks that write
-			// nothing are left alone ----
+			// nothing are left alone. MASKED scales a masked layer's weight per bone and weighs ADDITIVE layers ----
 			if constexpr (LAYERED)
 			{
 				__syncthreads();
@@ -304,10 +330,20 @@ namespace aclb200
 					uint8_t* row = s_out + size_t(base) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
 					for (uint32_t layer = base + 1; layer < (stack + 1) * p.num_layers; ++layer)
 					{
-						const uint32_t op = s_layer[layer].op;
-						const uint8_t* layer_row = s_out + size_t(layer) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
+						const uint32_t slot = s_layer[layer].op;
+						const uint32_t op = slot_op(slot);
+						float weight = s_layer[layer].weight;
+						if (MASKED && slot > k_layer_op_mask)
+						{
+							// the layer's weight at this bone is weight * mask[bone]; a mask of +-0 leaves the running row as it is
+							const float mask = __ldg(p.bone_masks + ((slot >> k_layer_op_bits) - 1) * p.mask_stride + bone);
+							if (mask == 0.0f)
+								continue;
+							weight = __fmul_rn(weight, mask);
+						}
+						uint8_t* layer_row = s_out + size_t(layer) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
 						if (op == ACLB200_LAYER_BLEND)
-							obj::blend_row(row, row, layer_row, s_layer[layer].weight, p.layout == ACLB200_LAYOUT_QVV40);
+							obj::blend_row(row, row, layer_row, weight, p.layout == ACLB200_LAYOUT_QVV40);
 						else if (op == ACLB200_LAYER_ADDITIVE)
 						{
 							uint32_t format = p.additive_format;
@@ -315,6 +351,14 @@ namespace aclb200
 							{
 								format = __ldg(p.clip_additive_formats + s_req[layer].clip);
 								format = format <= ACLB200_ADDITIVE_ADDITIVE1 ? format : ACLB200_ADDITIVE_NONE;		// apply_additive_to_base's `default:`
+							}
+							// MASKED, weight != 1: the layer's row becomes qvv_lerp(writer defaults, layer, weight) in place (no other thread
+							// reads it), which scales the additive delta of every format
+							if (MASKED && weight != 1.0f)
+							{
+								const bool qvv40 = p.layout == ACLB200_LAYOUT_QVV40;
+								const float* defaults = k_writer_default_rows[qvv40][(s_req[layer].clip_flags & k_clip_default_scale_one) != 0];
+								obj::blend_row(layer_row, reinterpret_cast<const uint8_t*>(defaults), layer_row, weight, qvv40);
 							}
 							// (a flag is rare: reported where it is met, so that no accumulator stays live through the fold)
 							const uint32_t flags = obj::apply_additive_row(row, row, layer_row, format, p.layout == ACLB200_LAYOUT_QVV40);
@@ -1058,7 +1102,7 @@ namespace aclb200
 	{
 		const bool force_output_staging = compose != k_compose_local;
 		const bool pairs = compose == k_compose_additive || compose == k_compose_blend;
-		const bool layers = compose == k_compose_layers;
+		const bool layers = compose == k_compose_layers || compose == k_compose_layers_masked;
 		const uint32_t state_bytes = (database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState))) + (layers ? uint32_t(sizeof(LayerSlot)) : 0u);
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);

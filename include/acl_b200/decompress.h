@@ -493,6 +493,29 @@ namespace acl_b200
 				additive_format, d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream),
 				"aclb200_decompress_tracks_layered_skinning");
 		}
+		// Masked layer stacks (aclb200_decompress_tracks_layered_masked): decompress_tracks_layered where layer i of pose r may name a bone
+		// mask d_layer_masks[r * num_layers + i] (ACLB200_LAYER_NO_MASK: none; d_layer_masks nullptr: no masks), mask m being
+		// d_bone_masks[m * mask_stride + b] per bone b of the base clip (mask_stride 0: max_tracks). At bone b the layer's weight is
+		// weight * mask[b], and a mask of +-0 leaves the bone untouched; ADDITIVE layers take their weight (the additive delta lerped from the
+		// track_writer defaults when it is not 1). ADDITIVE weights 1 without masks give decompress_tracks_layered's bytes.
+		void decompress_tracks_layered_masked(const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers,
+			const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options& options, uint32_t additive_format,
+			const uint8_t* d_clip_additive_formats, void* d_out, const uint32_t* d_parent_indices = nullptr, const uint32_t* d_skeleton_offsets = nullptr,
+			uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_layered_masked(m_device->get(), m_clipset, d_layers, d_layer_masks, num_poses, num_layers,
+				d_bone_masks, num_masks, mask_stride, &options, additive_format, d_clip_additive_formats, d_parent_indices, d_skeleton_offsets,
+				object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_layered_masked");
+		}
+		void decompress_tracks_layered_masked_skinning(const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses,
+			uint32_t num_layers, const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options& options,
+			uint32_t additive_format, const uint8_t* d_clip_additive_formats, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+			const float* d_inverse_bind, void* d_out, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_layered_masked_skinning(m_device->get(), m_clipset, d_layers, d_layer_masks, num_poses,
+				num_layers, d_bone_masks, num_masks, mask_stride, &options, additive_format, d_clip_additive_formats, d_parent_indices,
+				d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_layered_masked_skinning");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

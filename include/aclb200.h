@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 10
+#define ACLB200_VERSION_MINOR 11
 
 typedef enum aclb200_status
 {
@@ -549,7 +549,8 @@ typedef struct aclb200_layer
 {
 	aclb200_request pose;			/* this layer's clip and sample time */
 	uint32_t op;					/* ACLB200_LAYER_* */
-	float    weight;				/* BLEND: the rtm::qvv_lerp weight, used as given (no clamp); ignored otherwise */
+	float    weight;				/* BLEND: the rtm::qvv_lerp weight, used as given (no clamp); ADDITIVE: ignored by
+									   aclb200_decompress_tracks_layered, the weight of the delta in _layered_masked; ignored otherwise */
 } aclb200_layer;
 
 /* A pose graph of up to eight clips per pose in one kernel: every layer is decoded, and the layers are folded into the running pose in
@@ -593,6 +594,46 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_layered(aclb200_context* co
  * clip]). Refusals as aclb200_decompress_tracks_layered, plus NULL parents and NULL or misaligned inverse binds. */
 ACLB200_API aclb200_status aclb200_decompress_tracks_layered_skinning(aclb200_context* context, const aclb200_clipset* clipset,
 	const aclb200_layer* d_layers, uint32_t num_poses, uint32_t num_layers, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The mask index of a layer without a bone mask (aclb200_decompress_tracks_layered_masked) */
+#define ACLB200_LAYER_NO_MASK 0xFFFFFFFFu
+
+/* Masked layer stacks: aclb200_decompress_tracks_layered with a per-bone weight mask on any layer (partial-body layers: an upper-body
+ * aim over lower-body locomotion, a wave on one arm, a feathered spine) and ADDITIVE layers that take their weight, in one kernel.
+ * Everything not listed here is as aclb200_decompress_tracks_layered (and _layered_skinning): base, OFF layers, decode, formats,
+ * policies, d_out, object kinds, skeletons, inverse binds, d_out_flags, database tiers, ACLB200_MATH_FAST, the shared memory limits.
+ *   d_layer_masks  device uint32[num_poses * num_layers] or NULL (no layer has a mask): d_layer_masks[r * num_layers + i] is the mask
+ *                  index of layer i of pose r, ACLB200_LAYER_NO_MASK for none. The mask index of an OFF layer or of the base is not read.
+ *   d_bone_masks   device float[num_masks * mask_stride], 4 byte aligned: mask m is d_bone_masks[m * mask_stride + b], one float per bone b
+ *                  of the BASE clip's skeleton (mask_stride 0: the clip set's max_tracks). Masks belong to a rig: a launch that mixes rigs
+ *                  names the right mask per layer.
+ *   weight at b    w_b = weight * mask[b] (one IEEE multiply), or weight for a layer without a mask. A mask value of +0 or -0 leaves
+ *                  bone b untouched, byte for byte: the bones outside a mask are those of the stack without the layer.
+ *   BLEND          running = rtm::qvv_lerp(running, layer, w_b) as aclb200_decompress_tracks_blend computes it; w_b used as given.
+ *   ADDITIVE       w_b == 1: running = acl::apply_additive_to_base(format, running, layer), what _layered computes. Otherwise
+ *                  running = acl::apply_additive_to_base(format, running, rtm::qvv_lerp(identity, layer, w_b)), identity = the track_writer
+ *                  default pose the layer is decoded with (identity rotation, zero translation, the clip's default scale: 1, or 0 for
+ *                  additive1 clips), the identity of every format: w_b scales the additive delta. Weight 0 is applied (an identity
+ *                  delta), a mask of 0 skips.
+ *   writes nothing as aclb200_decompress_tracks_layered, and also when a BLEND or ADDITIVE layer above the base names a mask index at or
+ *                  above num_masks (other than ACLB200_LAYER_NO_MASK).
+ * Migration: with every ADDITIVE weight set to 1 and no masks (d_layer_masks NULL), the outputs equal aclb200_decompress_tracks_layered's
+ * byte for byte.
+ * Refused, writing nothing and leaving *d_out_flags untouched: what aclb200_decompress_tracks_layered (_layered_skinning) refuses, and
+ * with d_layer_masks given: d_bone_masks NULL or not 4 byte aligned, num_masks 0 or above 2^29 - 1, a mask_stride below max_tracks,
+ * num_masks * mask_stride above 2^32 - 1 (ACLB200_ERR_INVALID_ARGUMENT). */
+ACLB200_API aclb200_status aclb200_decompress_tracks_layered_masked(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers,
+	const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options* options,
+	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+ACLB200_API aclb200_status aclb200_decompress_tracks_layered_masked_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_layer* d_layers, const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers,
+	const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options* options,
 	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
