@@ -18,4 +18,5 @@ from .api import (  # noqa: F401
     ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1, ADDITIVE_REQUEST_DTYPE, make_additive_requests,
     BLEND_REQUEST_DTYPE, make_blend_requests,
     LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE, LAYER_NO_MASK, MAX_LAYERS, LAYER_DTYPE, make_layers,
+    NO_BONE, MAX_QUERY_BONES,
 )

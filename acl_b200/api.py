@@ -173,6 +173,7 @@ def _lib():
                                                                vp, vp, vp]
         l.aclb200_decompress_tracks_layered_masked_skinning.argtypes = [vp, vp, vp, vp, u32, u32, vp, u32, u32, C.POINTER(Options), u32, vp, vp,
                                                                         vp, vp, vp, vp, vp]
+        l.aclb200_decompress_bones.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, u32, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -203,7 +204,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_blend", "aclb200_blend_poses", "aclb200_decompress_tracks_skinning",
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
-        "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning",
+        "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
     ]
 
 
@@ -248,6 +249,8 @@ def make_blend_requests(from_clips, from_times, to_clips, to_times) -> np.ndarra
 LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE = 0, 1, 2
 MAX_LAYERS = 8
 LAYER_NO_MASK = 0xFFFFFFFF      # the mask index of a layer without a bone mask (decompress_tracks_layered_masked)
+MAX_QUERY_BONES = 32             # bones per list of decompress_bones
+NO_BONE = 0xFFFFFFFF             # an unused entry of a bone list (decompress_bones)
 LAYER_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("op", np.uint32), ("weight", np.float32)])
 
 
@@ -502,6 +505,21 @@ class Context:
                                                                     C.byref(options), additive_format, _device_ptr(d_clip_additive_formats),
                                                                     _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
                                                                     _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def decompress_bones(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_bone_lists, bones_per_list: int, d_out,
+                         num_lists: int = 1, d_request_lists=None, d_parent_indices=None, kind: int = 0, d_skeleton_offsets=None,
+                         d_out_flags=None, stream=None) -> None:
+        """Chosen bones of each request: d_bone_lists holds num_lists lists of bones_per_list (K, 1..32) uint32 bone indices (NO_BONE: a
+        hole), request r uses list d_request_lists[r] (uint32, None: list 0 for every request). Entry j of request r's list lands at
+        d_out + r * pose_stride + j * bone size (pose_stride: options.pose_stride_bytes, 0 = K rows). Without d_parent_indices, row j is
+        row list[j] of decompress_tracks (options.output_layout); with them, row list[j] of decompress_tracks_object_space as `kind` rows,
+        clip c's skeleton at d_parent_indices + d_skeleton_offsets[c]. Only the listed bones' ancestor chains are decoded and walked. An
+        entry that is NO_BONE or beyond the clip's bones, a list index >= num_lists and an invalid clip leave their rows untouched.
+        d_out_flags: optional uint32 ERROR_FLAG_* of the walked bones."""
+        self._check(_lib().aclb200_decompress_bones(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
+                                                    _device_ptr(d_bone_lists), num_lists, bones_per_list, _device_ptr(d_request_lists),
+                                                    _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
+                                                    _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as

@@ -283,7 +283,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.11 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.12 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -343,7 +343,8 @@ extern "C"
 		context->device = device;
 		context->num_sms = prop.multiProcessorCount;
 		context->max_dynamic_smem = int(prop.sharedMemPerBlockOptin);
-		if (prop.major != 9 || prop.minor != 0 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess)
+		if (prop.major != 9 || prop.minor != 0 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess
+			|| configure_bones_kernels(context->max_dynamic_smem) != cudaSuccess)
 		{
 			// the kernels are compiled for sm_90a only, which runs on compute capability 9.0 and nothing else
 			delete context;
@@ -671,6 +672,54 @@ extern "C"
 			return status;
 		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
 			k_object_skinning, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_bones(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		const std::string what = "decompress_bones";
+		if (bones_per_list == 0 || bones_per_list > ACLB200_MAX_QUERY_BONES)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": bones_per_list must be 1 to 32");
+		if (num_lists == 0 || d_bone_lists == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs at least one bone list (num_lists >= 1, d_bone_lists not NULL)");
+		// make_params refuses skip masks and `skipped` default modes for a composed decode; its pose stride check is the whole pose's, so
+		// the launch is described as a single track one and the stride of K rows is checked here
+		const Composed composed = { "decompress_bones", k_pose_unfit, k_compose_object, 1 };
+		DecodeParams params;
+		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, true, params, &composed);
+		if (status != ACLB200_OK)
+			return status;
+		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": unknown object_kind");
+		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": object space output needs the QVV48 layout");
+		const uint64_t rows_bytes = uint64_t(bones_per_list) * params.bone_stride;
+		params.pose_stride = options->pose_stride_bytes != 0 ? options->pose_stride_bytes : rows_bytes;
+		if (params.pose_stride < rows_bytes)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": pose_stride_bytes is smaller than bones_per_list rows");
+		const bool database = params.db_tiers != nullptr;
+		BoneQuery query = {};
+		if (!plan_bones_launch(params, query, database, context->max_dynamic_smem))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, what + k_pose_unfit);
+		if (num_requests == 0)
+			return ACLB200_OK;
+		query.bone_lists = d_bone_lists;
+		query.request_lists = d_request_lists;
+		query.num_lists = num_lists;
+		query.bones_per_list = bones_per_list;
+		query.parent_indices = d_parent_indices;
+		query.skeleton_offsets = d_skeleton_offsets;
+		query.object_kind = object_kind;
+		query.out_flags = d_out_flags;
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, what.c_str());
+		if (cleared != ACLB200_OK)
+			return cleared;
+		return finish_launch(context, launch_decompress_bones(params, query, database, cuda_stream), database ? "decompress_bones (database)" : "decompress_bones");
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

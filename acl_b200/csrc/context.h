@@ -207,6 +207,28 @@ namespace aclb200
 		uint32_t mask_stride;
 	};
 
+	// The bone query (aclb200_decompress_bones, bones.cu): the lists, the skeletons and the launch's shared memory carve-up. A kernel
+	// argument of its own beside DecodeParams, which the other kernels share unchanged.
+	struct BoneQuery
+	{
+		const uint32_t* bone_lists;				// [num_lists][bones_per_list] bone indices, ACLB200_NO_BONE for a hole
+		const uint32_t* request_lists;			// [num_requests] the list of each request, or nullptr (every request takes list 0)
+		uint32_t num_lists;
+		uint32_t bones_per_list;				// K, 1..ACLB200_MAX_QUERY_BONES
+		const uint32_t* parent_indices;			// skeletons (object space rows), or nullptr (local rows)
+		const uint32_t* skeleton_offsets;		// [num_clips] first parent index of each clip's skeleton, or nullptr
+		uint32_t object_kind;					// ACLB200_OBJECT_QVVF or ACLB200_OBJECT_MATRIX3X4F, with parents
+		uint32_t* out_flags;					// ACLB200_ERROR_FLAG_* of the walked bones are OR-ed in, or nullptr
+		uint32_t requests_per_block;
+		uint32_t mask_words;					// closure bitmask words per request: ceil(max_tracks / 32)
+		uint32_t smem_pose_bytes;				// pose rows per request: max_tracks * bone size, 16 byte granular
+		uint32_t smem_words_offset;				// dynamic shared memory: request states | request words | closure bitmasks | work items |
+		uint32_t smem_mask_offset;				// pose rows
+		uint32_t smem_items_offset;
+		uint32_t smem_pose_offset;
+		uint32_t smem_bytes;
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
@@ -248,6 +270,10 @@ namespace aclb200
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_track(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t configure_kernels(int& max_dynamic_smem);
+	// bones.cu: the bone query. plan_bones_launch returns false when one request does not fit max_dynamic_smem.
+	cudaError_t configure_bones_kernels(int max_dynamic_smem);
+	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem);
+	cudaError_t launch_decompress_bones(const DecodeParams& params, const BoneQuery& query, bool database, cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

@@ -516,6 +516,17 @@ namespace acl_b200
 				num_layers, d_bone_masks, num_masks, mask_stride, &options, additive_format, d_clip_additive_formats, d_parent_indices,
 				d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_layered_masked_skinning");
 		}
+		// Bone queries (aclb200_decompress_bones): entry j of request r's bone list (list d_request_lists[r], or list 0 when it is nullptr;
+		// list l is d_bone_lists[l * bones_per_list ..], ACLB200_NO_BONE for a hole) lands at d_out + r * pose_stride + j * bone size. Without
+		// parents, row list[j] of decompress_tracks; with them, row list[j] of decompress_tracks_object_space as object_kind rows. Only the
+		// listed bones' ancestor chains are decoded and walked.
+		void decompress_bones(const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options& options, const uint32_t* d_bone_lists,
+			uint32_t num_lists, uint32_t bones_per_list, void* d_out, const uint32_t* d_request_lists = nullptr, const uint32_t* d_parent_indices = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_bones(m_device->get(), m_clipset, d_requests, num_requests, &options, d_bone_lists, num_lists, bones_per_list,
+				d_request_lists, d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_bones");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 11
+#define ACLB200_VERSION_MINOR 12
 
 typedef enum aclb200_status
 {
@@ -636,6 +636,44 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_layered_masked_skinning(acl
 	const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride, const aclb200_options* options,
 	uint32_t additive_format, const uint8_t* d_clip_additive_formats,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The bones per list of aclb200_decompress_bones, and an unused entry of a bone list */
+#define ACLB200_MAX_QUERY_BONES 32
+#define ACLB200_NO_BONE 0xFFFFFFFFu
+
+/* Bone queries: chosen bones of each pose (attachment sockets, IK effectors and feet, motion matching features, the root), in one kernel
+ * that decodes and walks only the ancestor chains of the requested bones and stores only the requested rows.
+ *   bone lists      K = bones_per_list (1..ACLB200_MAX_QUERY_BONES); list l is d_bone_lists[l * K .. l * K + K - 1] (device). Request r
+ *                   uses list d_request_lists[r] (device uint32[num_requests]), or list 0 for every request when d_request_lists is NULL.
+ *                   A list may hold duplicates, any order and ACLB200_NO_BONE holes. A request whose list index is >= num_lists writes
+ *                   nothing.
+ *   d_out           entry j of request r's list at d_out + r * pose_stride + j * bone size; pose_stride = options->pose_stride_bytes, 0 =
+ *                   K * bone size (48 bytes, or 40 for local QVV40 rows); alignment as aclb200_decompress_tracks requires for the layout.
+ *                   An entry that is ACLB200_NO_BONE, or at or above its clip's num_tracks, leaves its row untouched (as
+ *                   aclb200_decompress_track does with an invalid track index). A request with an invalid clip index writes nothing.
+ *   local rows      d_parent_indices NULL: row j is row list[j] of what aclb200_decompress_tracks computes for the request with the same
+ *                   options, in options->output_layout (QVV48 or QVV40), byte for byte. Only the listed bones are decoded, with
+ *                   aclb200_decompress_tracks's arithmetic (not aclb200_decompress_track's normalisation).
+ *   object rows     d_parent_indices given: row j is row list[j] of aclb200_decompress_tracks_object_space for the same request, options,
+ *                   skeleton (d_parent_indices + d_skeleton_offsets[clip], d_skeleton_offsets NULL: 0) and object_kind
+ *                   (ACLB200_OBJECT_QVVF or ACLB200_OBJECT_MATRIX3X4F; QVV48 only), byte for byte. Only the bones on the listed bones'
+ *                   ancestor chains are decoded and walked. A parent that does not precede its child ends the chain and its bone is
+ *                   treated as a root, as the whole walk does: the ancestor walk only ever moves to a lower bone index, so it ends on any
+ *                   parent table.
+ *   d_out_flags     device uint32, optional: cleared, then the ACLB200_ERROR_FLAG_* met on the walked bones OR-ed in. This can be fewer
+ *                   bits than aclb200_decompress_tracks_object_space reports for the same poses: a mirrored bone or a bad parent outside
+ *                   every chain is not walked.
+ * As aclb200_decompress_tracks_object_space: per request and per track policies, default modes and variable defaults, a bound database's
+ * streamed tiers; every operation IEEE and unfused, ACLB200_MATH_FAST accepted and runs the exact decode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, writing nothing and leaving *d_out_flags untouched: bones_per_list 0 or above 32, num_lists 0,
+ * NULL d_bone_lists, skip masks or a `skipped` default mode, a scalar clip set, with parents an unknown object_kind or QVV40, a pose stride
+ * below K * bone size, the alignment rules of aclb200_decompress_tracks. ACLB200_ERR_UNSUPPORTED when one pose of the widest clip does not
+ * fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_bones(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
 
 /* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
