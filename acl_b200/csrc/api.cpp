@@ -362,6 +362,8 @@ extern "C"
 		cudaFree(context->d_scratch_requests);
 		cudaFree(context->d_scratch_out);
 		cudaFree(context->d_error_scratch);
+		if (context->error_scratch_done != nullptr)
+			cudaEventDestroy(context->error_scratch_done);
 		if (context->host_stream != nullptr)
 			cudaStreamDestroy(context->host_stream);
 		if (context->copy_stream != nullptr)

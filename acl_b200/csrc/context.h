@@ -32,6 +32,7 @@ struct aclb200_context
 	// aclb200_calculate_compression_error (error_metric.cu): job table, arg max accumulators, requests and the decoded poses of one chunk
 	void* d_error_scratch = nullptr;
 	size_t error_scratch_bytes = 0;
+	cudaEvent_t error_scratch_done = nullptr;	// recorded after the last kernel of a call that reads the scratch, on that call's stream
 	uint64_t error_chunk_bytes = 1024ull << 20;	// decoded poses per chunk (aclb200_set_error_chunk_bytes)
 
 	// aclb200_debug_set_trace

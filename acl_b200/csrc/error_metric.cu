@@ -516,19 +516,44 @@ namespace aclb200
 			return uint32_t(std::min<size_t>(8, block_budget / per_warp));
 		}
 
+		// The context's scratch is shared by every call, whatever its stream: a call makes its stream wait for the previous user's last
+		// reader before it writes (error_scratch_done), and records the event after its own last reader (ScratchUse).
 		aclb200_status grow_scratch(aclb200_context* context, size_t bytes)
 		{
+			if (context->error_scratch_done == nullptr)
+			{
+				const cudaError_t error = cudaEventCreateWithFlags(&context->error_scratch_done, cudaEventDisableTiming);
+				if (error != cudaSuccess)
+				{
+					context->error_scratch_done = nullptr;
+					return check_cuda(context, error, "error scratch: event creation");
+				}
+			}
 			if (context->error_scratch_bytes >= bytes)
 				return ACLB200_OK;
+			// the old buffer may still be read by a call on another stream
+			cudaError_t error = cudaEventSynchronize(context->error_scratch_done);
+			if (error != cudaSuccess)
+				return check_cuda(context, error, "error scratch: waiting for its last reader");
 			cudaFree(context->d_error_scratch);
 			context->d_error_scratch = nullptr;
 			context->error_scratch_bytes = 0;
-			const cudaError_t error = cudaMalloc(&context->d_error_scratch, bytes);
+			error = cudaMalloc(&context->d_error_scratch, bytes);
 			if (error != cudaSuccess)
 				return check_cuda(context, error, "calculate_compression_error: scratch allocation");
 			context->error_scratch_bytes = bytes;
 			return ACLB200_OK;
 		}
+
+		// From the stream's wait to the end of the call: every return records the scratch's last use on the call's stream, after whatever
+		// it enqueued.
+		struct ScratchUse
+		{
+			aclb200_context* context;
+			cudaStream_t stream;
+			cudaError_t wait() const { return cudaStreamWaitEvent(stream, context->error_scratch_done, 0); }
+			~ScratchUse() { cudaEventRecord(context->error_scratch_done, stream); }
+		};
 
 		size_t align_up(size_t value, size_t alignment) { return (value + alignment - 1) / alignment * alignment; }
 	}
@@ -732,8 +757,11 @@ extern "C"
 		uint8_t* d_lossy = scratch + jobs_bytes + keys_bytes + flags_bytes + requests_bytes + pose_jobs_bytes;
 
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		const ScratchUse use{ context, cuda_stream };
+		cudaError_t error = use.wait();
 		// pageable source: the copy has left `ordered` when the call returns
-		cudaError_t error = cudaMemcpyAsync(d_jobs, ordered.data(), sizeof(ErrorJobDev) * ordered.size(), cudaMemcpyHostToDevice, cuda_stream);
+		if (error == cudaSuccess)
+			error = cudaMemcpyAsync(d_jobs, ordered.data(), sizeof(ErrorJobDev) * ordered.size(), cudaMemcpyHostToDevice, cuda_stream);
 		if (error == cudaSuccess)
 			error = cudaMemsetAsync(d_keys, 0, keys_bytes + flags_bytes, cuda_stream);
 		if (error != cudaSuccess)
@@ -872,7 +900,10 @@ extern "C"
 			return grown;
 		uint8_t* scratch = static_cast<uint8_t*>(context->d_error_scratch);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		cudaError_t error = cudaMemcpyAsync(scratch, ordered.data(), sizeof(ErrorJobDev) * ordered.size(), cudaMemcpyHostToDevice, cuda_stream);
+		const ScratchUse use{ context, cuda_stream };
+		cudaError_t error = use.wait();
+		if (error == cudaSuccess)
+			error = cudaMemcpyAsync(scratch, ordered.data(), sizeof(ErrorJobDev) * ordered.size(), cudaMemcpyHostToDevice, cuda_stream);
 		if (error != cudaSuccess)
 			return check_cuda(context, error, "decompress_all_samples: job upload");
 

@@ -360,6 +360,9 @@ typedef struct aclb200_error_job
  *                     pose_stride_bytes / 48 floats (= max_tracks by default; scalar clip sets: tracks per row)
  * rtm::quat_normalize's rsqrtss estimate is CPU specific: errors agree with a given CPU's
  * within 5e-5 on poses tens of units across, not bit for bit (see error_metric.cu). Asynchronous on `stream`; uses scratch owned by the context.
+ * That scratch is shared with aclb200_decompress_all_samples: each call's work on `stream` waits for the previous such call on the
+ * context to finish reading it, on whatever stream that call ran, so calls on different streams run one after the other on the device
+ * (never at the same time), and a call that has to grow the scratch first waits on the host for that previous call.
  * A clip set whose bound database has chunks streamed in is refused with ACLB200_ERR_UNSUPPORTED: these measurements never ignore tiers. */
 ACLB200_API aclb200_status aclb200_calculate_compression_error(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_error_job* jobs,
 	uint32_t num_jobs, const void* d_raw_poses, const uint32_t* d_parent_indices, const float* d_shell_distances,
@@ -371,7 +374,8 @@ ACLB200_API aclb200_status aclb200_calculate_compression_error(aclb200_context* 
  * Job j contributes num_samples poses, sample i sought at min(i / sample_rate, duration) with options->rounding_policy (the reference
  * uses `nearest` "to land directly on a sample") and decoded like aclb200_decompress_tracks / aclb200_scalar_decompress_tracks would:
  * the poses of the jobs follow one another in d_out (pose stride and layout from `options`). Only clip, num_samples, sample_rate and
- * duration of a job are read. jobs is a HOST array; asynchronous on `stream`; uses scratch owned by the context.
+ * duration of a job are read. jobs is a HOST array; asynchronous on `stream`; uses scratch owned by the context, ordered after the
+ * previous call that used it on any stream (see aclb200_calculate_compression_error).
  * ACLB200_ERR_UNSUPPORTED on a clip set whose bound database has chunks streamed in. */
 ACLB200_API aclb200_status aclb200_decompress_all_samples(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_error_job* jobs,
 	uint32_t num_jobs, const aclb200_options* options, void* d_out, void* stream);
