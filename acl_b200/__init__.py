@@ -13,10 +13,11 @@ from .api import (  # noqa: F401
     DEFAULT_SKIPPED, DEFAULT_CONSTANT, DEFAULT_VARIABLE, DEFAULT_LEGACY,
     LAYOUT_QVV48, LAYOUT_QVV40, MATH_EXACT, MATH_FAST, TRACK_QVVF,
     SKIP_ROTATION, SKIP_TRANSLATION, SKIP_SCALE,
-    ERROR_JOB_DTYPE, TRACK_ERROR_DTYPE, ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON,
+    ERROR_JOB_DTYPE, TRACK_ERROR_DTYPE, ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON, ERROR_FLAG_WRAP_CLIP_CYCLE,
     OBJECT_QVVF, OBJECT_MATRIX3X4F,
     ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1, ADDITIVE_REQUEST_DTYPE, make_additive_requests,
     BLEND_REQUEST_DTYPE, make_blend_requests,
     LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE, LAYER_NO_MASK, MAX_LAYERS, LAYER_DTYPE, make_layers,
     NO_BONE, MAX_QUERY_BONES,
+    MAX_ROOT_MOTION_CYCLES, ROOT_MOTION_REQUEST_DTYPE, make_root_motion_requests,
 )

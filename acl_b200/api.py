@@ -36,7 +36,7 @@ ERROR_JOB_DTYPE = np.dtype([("clip", np.uint32), ("num_samples", np.uint32), ("s
 METRIC_QVVF, METRIC_QVVF_MATRIX3X4F = 0, 1
 ADDITIVE_NONE, ADDITIVE_RELATIVE, ADDITIVE_ADDITIVE0, ADDITIVE_ADDITIVE1 = 0, 1, 2, 3
 TRACK_ERROR_DTYPE = np.dtype([("index", np.uint32), ("error", np.float32), ("sample_time", np.float32), ("flags", np.uint32)])
-ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON = 1, 2
+ERROR_FLAG_NEGATIVE_SCALE, ERROR_FLAG_INVALID_SKELETON, ERROR_FLAG_WRAP_CLIP_CYCLE = 1, 2, 4
 OBJECT_QVVF, OBJECT_MATRIX3X4F = 0, 1
 
 
@@ -174,6 +174,7 @@ def _lib():
         l.aclb200_decompress_tracks_layered_masked_skinning.argtypes = [vp, vp, vp, vp, u32, u32, vp, u32, u32, C.POINTER(Options), u32, vp, vp,
                                                                         vp, vp, vp, vp, vp]
         l.aclb200_decompress_bones.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, u32, vp, vp, vp, u32, vp, vp, vp]
+        l.aclb200_extract_root_motion.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -205,6 +206,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
         "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
+        "aclb200_extract_root_motion",
     ]
 
 
@@ -252,6 +254,9 @@ LAYER_NO_MASK = 0xFFFFFFFF      # the mask index of a layer without a bone mask 
 MAX_QUERY_BONES = 32             # bones per list of decompress_bones
 NO_BONE = 0xFFFFFFFF             # an unused entry of a bone list (decompress_bones)
 LAYER_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("op", np.uint32), ("weight", np.float32)])
+MAX_ROOT_MOTION_CYCLES = 256     # the most loop boundaries one extract_root_motion request may cross
+# numpy view of aclb200_root_motion_request {uint32 clip; float from_time; float to_time; int32 cycles}
+ROOT_MOTION_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("from_time", np.float32), ("to_time", np.float32), ("cycles", np.int32)])
 
 
 def make_layers(clips, times, ops, weights) -> np.ndarray:
@@ -265,6 +270,19 @@ def make_layers(clips, times, ops, weights) -> np.ndarray:
     out["op"] = ops
     out["weight"] = weights
     return out
+
+
+def make_root_motion_requests(clips, from_times, to_times, cycles=0) -> np.ndarray:
+    """(clip index, previous playback time, current playback time, loop boundaries crossed) arrays, or anything that broadcasts to one
+    shape -> aclb200_root_motion_request[]"""
+    clips, from_times, to_times, cycles = np.broadcast_arrays(np.asarray(clips, dtype=np.uint32), np.asarray(from_times, dtype=np.float32),
+                                                              np.asarray(to_times, dtype=np.float32), np.asarray(cycles, dtype=np.int32))
+    out = np.empty(clips.shape, dtype=ROOT_MOTION_REQUEST_DTYPE)
+    out["clip"] = clips
+    out["from_time"] = from_times
+    out["to_time"] = to_times
+    out["cycles"] = cycles
+    return out.reshape(-1)
 
 
 def _device_ptr(x) -> int:
@@ -520,6 +538,18 @@ class Context:
                                                     _device_ptr(d_bone_lists), num_lists, bones_per_list, _device_ptr(d_request_lists),
                                                     _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
                                                     _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def extract_root_motion(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, d_root_tracks=None,
+                            d_out_flags=None, stream=None) -> None:
+        """Root motion of num_requests make_root_motion_requests: M of request r is one 48 byte rtm::qvvf row at d_out + r * 48, the
+        delta with T(to) = qvv_mul(M, T(from)) when cycles == 0, composed across `cycles` loop boundaries otherwise (T(t): the root
+        track's decompress_tracks row at t with the clamp policy; the root of clip c is d_root_tracks[c], uint32, None: track 0).
+        options need the QVV48 layout and LOOP_CLAMP. An invalid clip, a root beyond the clip's tracks or |cycles| >
+        MAX_ROOT_MOTION_CYCLES leaves the row untouched. d_out_flags: optional uint32, ERROR_FLAG_NEGATIVE_SCALE (a mirrored root) and
+        ERROR_FLAG_WRAP_CLIP_CYCLE (cycles != 0 on a clip compressed with the wrap policy)."""
+        self._check(_lib().aclb200_extract_root_motion(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
+                                                       _device_ptr(d_root_tracks), _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                       _stream_ptr(stream)))
 
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as

@@ -46,15 +46,24 @@ namespace aclb200
 		const char* const k_pair_unfit = ": the two poses of a pair do not fit in a block's shared memory";
 		const char* const k_layers_unfit = ": the poses of a layer stack do not fit in a block's shared memory";
 
-		// composed: the description of a composed decode, nullptr for the plain decode
-		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
-			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			const Composed* composed = nullptr)
+		// what every decode checks before it reads an option: the handles, and an options struct of this library's size
+		aclb200_status check_handles_and_options(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_options* options)
 		{
 			if (context == nullptr || clipset == nullptr || options == nullptr)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
 			if (options->struct_size != sizeof(aclb200_options))
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "options.struct_size does not match this library, call aclb200_default_options()");
+			return ACLB200_OK;
+		}
+
+		// composed: the description of a composed decode, nullptr for the plain decode
+		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
+			const Composed* composed = nullptr)
+		{
+			const aclb200_status checked = check_handles_and_options(context, clipset, options);
+			if (checked != ACLB200_OK)
+				return checked;
 			if (num_requests != 0 && (d_requests == nullptr || d_out == nullptr))
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null request / output pointer");
 			if (clipset->device != context->device)
@@ -283,7 +292,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.12 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.13 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -722,6 +731,45 @@ extern "C"
 		if (cleared != ACLB200_OK)
 			return cleared;
 		return finish_launch(context, launch_decompress_bones(params, query, database, cuda_stream), database ? "decompress_bones (database)" : "decompress_bones");
+	}
+
+	aclb200_status aclb200_extract_root_motion(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_root_motion_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const uint32_t* d_root_tracks, void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		static_assert(sizeof(aclb200_root_motion_request) == 16, "a root motion request is one 16 byte load");
+		const std::string what = "extract_root_motion";
+		// the handles and the options struct's size before any option is read or the struct is copied
+		const aclb200_status checked = check_handles_and_options(context, clipset, options);
+		if (checked != ACLB200_OK)
+			return checked;
+		if (options->output_layout != ACLB200_LAYOUT_QVV48)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": the root samples and the output are QVV48 rows");
+		if (options->looping_policy != ACLB200_LOOP_CLAMP)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": every root sample is taken with the clamp looping policy");
+		if (options->d_request_policies != nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": per request policies would override the clamp looping policy");
+		// make_params refuses skip masks and `skipped` default modes for a composed decode, a scalar clip set, NULL pointers and a misaligned
+		// output; the rows are 48 bytes apart whatever pose_stride_bytes says
+		aclb200_options row_options = *options;
+		row_options.pose_stride_bytes = 0;
+		const Composed composed = { "extract_root_motion", k_pose_unfit, k_compose_object, 1 };
+		DecodeParams params;
+		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), num_requests, &row_options,
+			d_out, true, true, params, &composed);
+		if (status != ACLB200_OK || num_requests == 0)
+			return status;
+		params.requests = nullptr;
+		params.pose_stride = 48;
+		const RootMotionQuery query = { d_requests, d_root_tracks, d_out_flags };
+		const bool database = params.db_tiers != nullptr;
+		cudaSetDevice(context->device);
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, what.c_str());
+		if (cleared != ACLB200_OK)
+			return cleared;
+		return finish_launch(context, launch_extract_root_motion(params, query, database, cuda_stream),
+			database ? "extract_root_motion (database)" : "extract_root_motion");
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

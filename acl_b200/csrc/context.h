@@ -230,6 +230,15 @@ namespace aclb200
 		uint32_t smem_bytes;
 	};
 
+	// Root motion (aclb200_extract_root_motion, root_motion.cu): the requests and the root track of each clip. A kernel argument of its own
+	// beside DecodeParams, whose `requests` it leaves unused (each lane builds its own request from the root motion request's times).
+	struct RootMotionQuery
+	{
+		const aclb200_root_motion_request* requests;
+		const uint32_t* root_tracks;			// [num_clips] the root track of each clip, or nullptr (track 0)
+		uint32_t* out_flags;					// ACLB200_ERROR_FLAG_NEGATIVE_SCALE and ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE are OR-ed in, or nullptr
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
@@ -275,6 +284,8 @@ namespace aclb200
 	cudaError_t configure_bones_kernels(int max_dynamic_smem);
 	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem);
 	cudaError_t launch_decompress_bones(const DecodeParams& params, const BoneQuery& query, bool database, cudaStream_t stream);
+	// root_motion.cu: root motion, one lane per (request, sample)
+	cudaError_t launch_extract_root_motion(const DecodeParams& params, const RootMotionQuery& query, bool database, cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

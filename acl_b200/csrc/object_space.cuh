@@ -3,7 +3,8 @@
 // qvv and 3x4 matrix operations in unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which
 // the error measurement, the additive decode (COMPOSE = k_compose_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which
 // the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share. And the skinning step, which the three composed decodes (with
-// the internal object kind k_object_skinning) and aclb200_local_to_skinning run after the matrix walk.
+// the internal object kind k_object_skinning) and aclb200_local_to_skinning run after the matrix walk. And rtm::qvv_inverse, which root motion
+// (root_motion.cu) composes with qvv_mul.
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
@@ -381,6 +382,23 @@ namespace aclb200
 					return qvv_mul_positive(fp, lhs, rhs);
 				Qvv<float> out;
 				qvv_mul_negative_scale(&lhs, &rhs, &out);
+				return out;
+			}
+
+			// rtm::qvv_inverse(input), qvvf.h:389-395, the one argument form (root motion, root_motion.cu): quat_conjugate (the sign bits of x, y
+			// and z xor-ed, quatf.h:482-491), vector_reciprocal as the IEEE division 1 / scale (_mm_div_ps, vector4f.h:1310), then
+			// -quat_mul_vector3(translation * inv_scale, inv_rotation) with vector_neg's sign xor (vector4f.h:1261-1271). No normalisation.
+			__device__ __forceinline__ Qvv<float> qvv_inverse(const Qvv<float>& input)
+			{
+				const Fp<float> fp{};
+				const auto neg = [](float v) { return __uint_as_float(__float_as_uint(v) ^ 0x80000000u); };
+				Qvv<float> out;
+				out.rotation = Quat<float>{ neg(input.rotation.x), neg(input.rotation.y), neg(input.rotation.z), input.rotation.w };
+				out.scale = Vec3<float>{ __fdiv_rn(1.0f, input.scale.x), __fdiv_rn(1.0f, input.scale.y), __fdiv_rn(1.0f, input.scale.z) };
+				const Vec3<float> scaled = { fp.mul(input.translation.x, out.scale.x), fp.mul(input.translation.y, out.scale.y),
+					fp.mul(input.translation.z, out.scale.z) };
+				const Vec3<float> rotated = quat_mul_vector3(fp, scaled, out.rotation);
+				out.translation = Vec3<float>{ neg(rotated.x), neg(rotated.y), neg(rotated.z) };
 				return out;
 			}
 

@@ -1,0 +1,178 @@
+// acl_b200/csrc/root_motion.cu -- root motion (aclb200_extract_root_motion): the root's displacement between two playback times of each
+// request, across loop boundaries, composed from root samples taken with the clamp policy.
+//
+// A request needs up to four samples of its clip's root track: T(from), T(to) and, when playback crossed a loop boundary, the clip's two
+// ends T(D) and T(0). Each sample is the root's row of aclb200_decompress_tracks for {clip, t}: the same seek (seek_request) and the same
+// device decoders with SINGLE = false (constant_sub_tracks, animated_rotation, animated_vector), restricted to one bone as the bone query
+// restricts them to its closure (bones.cu phase 3).
+//
+// Work decomposition, thread block = 64 requests, one lane per (request, sample slot), 8 requests per warp:
+//   slot 0 from_time, slot 1 to_time, slot 2 the clamp duration D, slot 3 time 0. The lane seeks its own time and decodes the root's three
+//   sub-tracks into a row in registers; the cycle end slots decode nothing when the request crosses no boundary.
+//   The request's slot 0 lane gathers the other three rows with __shfl_sync, composes M (rtm::qvv_inverse, rtm::qvv_mul in unfused IEEE
+//   operations, object_space.cuh) and stores its 48 byte row. No pose row goes through shared memory.
+#include "device_common.cuh"
+#include "object_space.cuh"
+
+#include <type_traits>
+
+namespace aclb200
+{
+	using namespace dev;
+
+	namespace
+	{
+		constexpr uint32_t k_root_motion_slots = 4;			// from, to, the clip's end (D), its start (0)
+		constexpr uint32_t k_root_motion_requests_per_block = k_threads_per_block / k_root_motion_slots;
+		static_assert(32 % k_root_motion_slots == 0, "a request's slots lie in one warp");
+
+		using obj::Qvv;
+		using obj::Quat;
+		using obj::Vec3;
+
+		// rtm::qvv_mul(lhs, rhs) through whichever branch it takes; the matrix branch (a mirrored root) is reported
+		__device__ __forceinline__ Qvv<float> qvv_mul_flagged(const Qvv<float>& lhs, const Qvv<float>& rhs, uint32_t& flags)
+		{
+			if (obj::takes_negative_branch(obj::Fp<float>{}, lhs.scale, rhs.scale))
+				flags |= ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
+			return obj::qvv_mul_any(lhs, rhs);
+		}
+
+		// the row of lane `source` of the warp, as an rtm::qvvf
+		__device__ __forceinline__ Qvv<float> shuffle_row(const float4 row[3], uint32_t source)
+		{
+			Qvv<float> q;
+			q.rotation = Quat<float>{ __shfl_sync(0xFFFFFFFFu, row[0].x, source), __shfl_sync(0xFFFFFFFFu, row[0].y, source),
+				__shfl_sync(0xFFFFFFFFu, row[0].z, source), __shfl_sync(0xFFFFFFFFu, row[0].w, source) };
+			q.translation = Vec3<float>{ __shfl_sync(0xFFFFFFFFu, row[1].x, source), __shfl_sync(0xFFFFFFFFu, row[1].y, source),
+				__shfl_sync(0xFFFFFFFFu, row[1].z, source) };
+			q.scale = Vec3<float>{ __shfl_sync(0xFFFFFFFFu, row[2].x, source), __shfl_sync(0xFFFFFFFFu, row[2].y, source),
+				__shfl_sync(0xFFFFFFFFu, row[2].z, source) };
+			return q;
+		}
+
+		template<int NORM, bool PER_TRACK, bool DB>
+		__global__ void __launch_bounds__(k_threads_per_block)
+		extract_root_motion_kernel(const DecodeParams p, const RootMotionQuery q)
+		{
+			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
+			const uint32_t lane = threadIdx.x & 31u;
+			const uint32_t slot = threadIdx.x & (k_root_motion_slots - 1);
+			const uint64_t request_index = uint64_t(blockIdx.x) * k_root_motion_requests_per_block + threadIdx.x / k_root_motion_slots;
+
+			// the request, its root track and whether it writes its row (an invalid clip, a root beyond the clip's tracks and too many
+			// cycles leave the row as it is)
+			uint32_t clip_index = 0xFFFFFFFFu;
+			float from_time = 0.0f, to_time = 0.0f;
+			int32_t cycles = 0;
+			if (request_index < p.num_requests)
+			{
+				// four 4 byte loads: the ABI only promises the request array the 4 byte alignment of its fields
+				const uint32_t* fields = reinterpret_cast<const uint32_t*>(q.requests + request_index);
+				clip_index = __ldg(fields);
+				from_time = __uint_as_float(__ldg(fields + 1));
+				to_time = __uint_as_float(__ldg(fields + 2));
+				cycles = int32_t(__ldg(fields + 3));
+			}
+			bool writes = false;
+			uint32_t root = 0, clip_flags = 0;
+			float duration = 0.0f;
+			if (clip_index < p.num_clips)
+			{
+				const ClipDesc& clip = p.clips[clip_index];
+				root = q.root_tracks != nullptr ? __ldg(q.root_tracks + clip_index) : 0u;
+				writes = root < clip.num_tracks && cycles >= -ACLB200_MAX_ROOT_MOTION_CYCLES && cycles <= ACLB200_MAX_ROOT_MOTION_CYCLES;
+				clip_flags = clip.flags;
+				duration = clip.duration_clamp;
+			}
+
+			// ---- one sample per lane: seek, then the root's constant, default and animated sub-tracks into a row in registers ----
+			float4 row[3] = { make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f) };
+			if (writes && (slot < 2 || cycles != 0))
+			{
+				const float time = slot == 0 ? from_time : slot == 1 ? to_time : slot == 2 ? duration : 0.0f;
+				RS rs;
+				seek_request<DB>(p, aclb200_request{ clip_index, time }, uint32_t(request_index), rs);
+				// the decoders write through a pointer, but at constant offsets of `row` once inlined: the row stays in registers (the kernel's
+				// local memory is only the argument block of the out-of-line negative scale path, obj::qvv_mul_negative_scale)
+				uint8_t* bone = reinterpret_cast<uint8_t*>(row);
+				const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + root);
+				constant_sub_tracks<NORM, false>(p, rs, root, desc, bone);
+				if ((uint32_t(desc) & 3) == 2)
+				{
+					float rotation[4];
+					animated_rotation<NORM, PER_TRACK, false, false>(p, rs, nullptr, (uint32_t(desc) >> 2) & k_bone_index_mask, rs.alpha, rotation);
+					write_rotation(p.layout, bone, rotation);
+				}
+#pragma unroll
+				for (uint32_t kind = 1; kind <= 2; ++kind)
+				{
+					const uint32_t bits = uint32_t(desc >> (k_bone_kind_shift * kind));
+					if ((bits & 3) == 2 && (kind == 1 || (rs.clip_flags & k_clip_has_scale)))
+					{
+						float value[3];
+						animated_vector<PER_TRACK, false, false>(p, rs, nullptr, kind, (bits >> 2) & k_bone_index_mask, rs.alpha, value);
+						write_vector(p.layout, bone, kind, value);
+					}
+				}
+			}
+
+			// ---- the request's slot 0 lane composes M from the four samples ----
+			const uint32_t first = lane & ~(k_root_motion_slots - 1);
+			const Qvv<float> from = shuffle_row(row, first);
+			const Qvv<float> to = shuffle_row(row, first + 1);
+			const Qvv<float> end = shuffle_row(row, first + 2);
+			const Qvv<float> start = shuffle_row(row, first + 3);
+			uint32_t flags = 0;
+			if (slot == 0 && writes)
+			{
+				Qvv<float> motion;
+				if (cycles == 0)
+					motion = qvv_mul_flagged(to, obj::qvv_inverse(from), flags);		// rel(from, to)
+				else
+				{
+					// forward: the boundary reached is the end, playback resumes at the start; backward the other way round
+					const bool forward = cycles > 0;
+					const Qvv<float> reached = forward ? end : start;
+					const Qvv<float> inverse_resumed = obj::qvv_inverse(forward ? start : end);
+					motion = qvv_mul_flagged(reached, obj::qvv_inverse(from), flags);				// rel(from, reached)
+					const Qvv<float> cycle = qvv_mul_flagged(reached, inverse_resumed, flags);		// rel(resumed, reached), once
+					const int32_t full_cycles = (forward ? cycles : -cycles) - 1;
+					for (int32_t i = 0; i < full_cycles; ++i)
+						motion = qvv_mul_flagged(cycle, motion, flags);
+					motion = qvv_mul_flagged(qvv_mul_flagged(to, inverse_resumed, flags), motion, flags);	// rel(resumed, to)
+					if (clip_flags & k_clip_wrap)
+						flags |= ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE;
+				}
+				obj::store_qvv_row(reinterpret_cast<float4*>(p.out + request_index * 48), motion);
+			}
+			flags = __reduce_or_sync(0xFFFFFFFFu, flags);
+			if (lane == 0 && flags != 0 && q.out_flags != nullptr)
+				atomicOr(q.out_flags, flags);
+		}
+
+		using RootMotionKernel = void (*)(DecodeParams, RootMotionQuery);
+
+		RootMotionKernel root_motion_kernel(uint32_t normalization, bool per_track, bool database)
+		{
+			const auto pick = [&](auto norm) -> RootMotionKernel {
+				constexpr int NORM = decltype(norm)::value;
+				if (per_track)
+					return database ? extract_root_motion_kernel<NORM, true, true> : extract_root_motion_kernel<NORM, true, false>;
+				return database ? extract_root_motion_kernel<NORM, false, true> : extract_root_motion_kernel<NORM, false, false>;
+			};
+			if (normalization == 0)
+				return pick(std::integral_constant<int, 0>());
+			if (normalization == 1)
+				return pick(std::integral_constant<int, 1>());
+			return pick(std::integral_constant<int, 2>());
+		}
+	}
+
+	cudaError_t launch_extract_root_motion(const DecodeParams& params, const RootMotionQuery& query, bool database, cudaStream_t stream)
+	{
+		const uint32_t blocks = uint32_t((uint64_t(params.num_requests) + k_root_motion_requests_per_block - 1) / k_root_motion_requests_per_block);
+		root_motion_kernel(params.normalization, params.per_track_rounding != 0, database)<<<blocks, k_threads_per_block, 0, stream>>>(params, query);
+		return cudaGetLastError();
+	}
+}

@@ -527,6 +527,15 @@ namespace acl_b200
 			m_device->check(aclb200_decompress_bones(m_device->get(), m_clipset, d_requests, num_requests, &options, d_bone_lists, num_lists, bones_per_list,
 				d_request_lists, d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_bones");
 		}
+		// Root motion (aclb200_extract_root_motion): the root's delta M between each request's from_time and to_time across `cycles` loop
+		// boundaries, one 48 byte rtm::qvvf row per request at d_out + r * 48; the root of clip c is d_root_tracks[c] (nullptr: track 0).
+		// options need the QVV48 layout and ACLB200_LOOP_CLAMP. An engine accumulates M as character = rtm::qvv_mul(M, character).
+		void extract_root_motion(const aclb200_root_motion_request* d_requests, uint32_t num_requests, const aclb200_options& options, void* d_out,
+			const uint32_t* d_root_tracks = nullptr, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_extract_root_motion(m_device->get(), m_clipset, d_requests, num_requests, &options, d_root_tracks, d_out, d_out_flags,
+				stream), "aclb200_extract_root_motion");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 12
+#define ACLB200_VERSION_MINOR 13
 
 typedef enum aclb200_status
 {
@@ -317,8 +317,10 @@ enum
 enum
 {
 	ACLB200_ERROR_FLAG_NEGATIVE_SCALE = 1,		/* informational: a negative scale took rtm::qvv_mul through its matrix branch (qvvf.h:320-345) somewhere */
-	ACLB200_ERROR_FLAG_INVALID_SKELETON = 2		/* a parent index does not precede its child (the reference reads an unwritten transform there):
+	ACLB200_ERROR_FLAG_INVALID_SKELETON = 2,	/* a parent index does not precede its child (the reference reads an unwritten transform there):
 												 * the bone was treated as a root */
+	ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE = 4		/* aclb200_extract_root_motion: a request crossed a loop boundary of a clip compressed with the
+												 * wrap policy, whose motion from its last sample back to its first is missing (see there) */
 };
 
 /* One clip to measure == one `calculate_compression_error(allocator, raw_tracks, context, error_metric)` call of the reference
@@ -679,6 +681,53 @@ ACLB200_API aclb200_status aclb200_decompress_bones(aclb200_context* context, co
 	const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* One root motion request: how far the root moved between two playback times of one clip */
+typedef struct aclb200_root_motion_request
+{
+	uint32_t clip;				/* index into the clip set */
+	float    from_time;			/* playback time at the previous update, seconds */
+	float    to_time;			/* playback time now */
+	int32_t  cycles;			/* loop boundaries crossed from from_time to to_time: 0 none; k > 0 playback ran forward past the clip's end
+								 * k times; k < 0 it ran backward past the start -k times */
+} aclb200_root_motion_request;
+
+/* The most loop boundaries one root motion request may cross */
+#define ACLB200_MAX_ROOT_MOTION_CYCLES 256
+
+/* Root motion: the root's displacement between the playback time of the previous update and the current one, across loop boundaries, in
+ * one launch. It moves the character, not the pose. The reference's clamp policy exists for this use: "This makes it possible to extract
+ * the total root motion by sampling at the full duration of the clip and at 0 seconds" (core/sample_looping_policy.h:47-55,
+ * docs/handling_looping_playback.md:22).
+ *   d_requests      device aclb200_root_motion_request[num_requests], 4 byte aligned (the alignment of its fields; no wider alignment is
+ *                   assumed).
+ *   root track      request r uses track d_root_tracks[clip] (device uint32[num_clips]), or track 0 when d_root_tracks is NULL.
+ *   T(t)            the root track's row of aclb200_decompress_tracks for the request {clip, t} with the same options, in QVV48, read as an
+ *                   rtm::qvvf. Every sample is taken with ACLB200_LOOP_CLAMP; times are clamped and rounded as aclb200_decompress_tracks
+ *                   does (the batch rounding policy, d_per_track_rounding). D is the clip's clamp duration (num_samples - 1) / sample_rate:
+ *                   T(D) is its last sample, T(0) its first.
+ *   rel(a, b)       rtm::qvv_mul(T(b), rtm::qvv_inverse(T(a))) (qvvf.h:315-355 with both branches; the one argument qvv_inverse,
+ *                   qvvf.h:389-395, whose vector_reciprocal is an IEEE division under SSE2, vector4f.h:1310). It is the delta with
+ *                   T(b) = qvv_mul(rel(a, b), T(a)), in the root's frame at a: an engine accumulates it as M <- qvv_mul(delta, M).
+ *   M               cycles == 0: rel(from, to), in either direction.
+ *                   cycles = k > 0: M = rel(from, D); then k - 1 times M = qvv_mul(rel(0, D), M); then M = qvv_mul(rel(0, to), M).
+ *                   cycles = k < 0: M = rel(from, 0); then -k - 1 times M = qvv_mul(rel(D, 0), M); then M = qvv_mul(rel(D, to), M).
+ *                   The full cycle delta is computed once per request; nothing is normalised beyond what rtm's functions do.
+ *   d_out           M of request r at d_out + r * 48 (16 byte aligned): rotation xyzw, translation xyz + 0, scale xyz + 0, the layout of
+ *                   ACLB200_OBJECT_QVVF rows. options->pose_stride_bytes is not used. A request with an invalid clip index, a root track
+ *                   at or beyond its clip's num_tracks or |cycles| > ACLB200_MAX_ROOT_MOTION_CYCLES leaves its row untouched.
+ *   d_out_flags     device uint32, optional: cleared, then OR-ed in: ACLB200_ERROR_FLAG_NEGATIVE_SCALE when a qvv_mul took its matrix
+ *                   branch (a mirrored root); ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE when a request that writes its row has cycles != 0 on a
+ *                   clip compressed with the wrap policy (aclb200_clip_info::looping_policy). Such a clip has no sample at its end, so
+ *                   the interval from its last sample back to its first contributes no motion: reported, not repaired.
+ * As aclb200_decompress_bones: a bound database's streamed tiers are read, variable defaults and the batch and per track rounding policies
+ * are honoured, ACLB200_MATH_FAST is accepted and runs the exact decode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing and leaving *d_out_flags untouched: NULL d_requests or d_out with
+ * num_requests > 0, d_out not 16 byte aligned, output_layout other than QVV48, looping_policy other than ACLB200_LOOP_CLAMP, a non-NULL
+ * d_request_policies (its looping byte would contradict the clamp rule), skip masks or a `skipped` default mode, a scalar clip set. */
+ACLB200_API aclb200_status aclb200_extract_root_motion(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_root_motion_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const uint32_t* d_root_tracks, void* d_out, uint32_t* d_out_flags, void* stream);
 
 /* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
  * aclb200_apply_additive_to_base): num_poses poses of rtm::qvvf rows of one skeleton (48 byte bones, 16 byte aligned, pose p at
