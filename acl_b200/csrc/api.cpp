@@ -56,10 +56,9 @@ namespace aclb200
 			return ACLB200_OK;
 		}
 
-		// composed: the description of a composed decode, nullptr for the plain decode
+		// The checks every decode shares and the DecodeParams they describe; a launch's own fields (its plan, its operands) are left 0
 		aclb200_status make_params(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_request* d_requests,
-			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params,
-			const Composed* composed = nullptr)
+			uint32_t num_requests, const aclb200_options* options, void* d_out, bool want_transform, bool single_track, DecodeParams& params)
 		{
 			const aclb200_status checked = check_handles_and_options(context, clipset, options);
 			if (checked != ACLB200_OK)
@@ -132,27 +131,37 @@ namespace aclb200
 			params.skip_tracks = is_transform ? options->d_skip_track_mask : nullptr;
 			params.request_policies = options->d_request_policies;
 			params.layout = options->output_layout;
-			// launches that keep the caller's bytes store sub-tracks straight to global memory instead of assembling whole poses in
-			// shared memory
-			const bool keeps_bytes = keeps_caller_bytes(*options);
-			const bool tracks_launch = is_transform && !single_track;
 			// a bound database with chunks streamed in: the launch takes the database kernels (with nothing streamed in, the resident key
 			// frames give the reference's result, so every other launch runs the kernels it always did)
-			const bool database = is_transform && database_streamed_in(clipset);
-			if (database)
+			if (is_transform && database_streamed_in(clipset))
 			{
 				params.db_first_segment = clipset->d_db_first_segment;
 				params.db_tiers = clipset->database->d_tiers;
 				params.db_bulk[0] = clipset->database->d_bulk[0];
 				params.db_bulk[1] = clipset->database->d_bulk[1];
 			}
-			// an object transform needs every sub-track of its parents, apply_additive_to_base and qvv_lerp every sub-track of both poses
-			if (composed != nullptr && keeps_bytes)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(composed->entry)
+			params.num_layers = 1;
+			return ACLB200_OK;
+		}
+
+		// an object transform needs every sub-track of its parents, apply_additive_to_base and qvv_lerp every sub-track of both poses:
+		// the composed decodes, the bone query and root motion refuse skip masks and `skipped` default modes
+		aclb200_status check_every_sub_track(aclb200_context* context, const aclb200_options& options, const std::string& entry)
+		{
+			if (keeps_caller_bytes(options))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry
 					+ ": the composed poses need every decoded sub-track (no skip masks, no `skipped` default mode)");
-			params.num_layers = composed != nullptr ? composed->num_layers : 1u;
-			plan_launch(params, tracks_launch ? clipset->max_key_frame_bytes : 0u, context->max_dynamic_smem, tracks_launch && !keeps_bytes, database,
-				composed != nullptr ? composed->compose : k_compose_local);
+			return ACLB200_OK;
+		}
+
+		// object space output (parents given): a known object kind, and QVV48 rows for the walk
+		aclb200_status check_object_output(aclb200_context* context, const aclb200_options& options, const uint32_t* d_parent_indices,
+			uint32_t object_kind, const std::string& entry)
+		{
+			if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": unknown object_kind");
+			if (d_parent_indices != nullptr && options.output_layout != ACLB200_LAYOUT_QVV48)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
 			return ACLB200_OK;
 		}
 
@@ -163,50 +172,17 @@ namespace aclb200
 			return check_cuda(context, error, what);
 		}
 
-		// The composed decodes: num_poses poses of composed.num_layers requests each at d_requests. Every refusal comes before the flags are
-		// cleared: a refused call writes nothing. d_inverse_bind is given by the skinning entry points only (they require parents), and
-		// makes the object kind k_object_skinning.
-		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const void* d_requests, uint32_t num_poses,
-			const aclb200_options* options, const Composed& composed, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
-			const float* d_inverse_bind, uint32_t object_kind, void* d_out, uint32_t* d_out_flags, void* stream)
+		// The tail of a launch that ORs ACLB200_ERROR_FLAG_* into d_out_flags: on the context's device, the flags word is cleared on the
+		// stream (a failure there is reported as `what`'s), then launch() runs and is counted when it started (reported as `route`'s)
+		template<class Launch>
+		aclb200_status launch_clearing_flags(aclb200_context* context, uint32_t* d_out_flags, cudaStream_t stream, const char* what, const char* route,
+			Launch launch)
 		{
-			const std::string entry = composed.entry;
-			DecodeParams params;
-			const aclb200_status status = make_params(context, clipset, static_cast<const aclb200_request*>(d_requests), num_poses * composed.num_layers,
-				options, d_out, true, false, params, &composed);
-			if (status != ACLB200_OK)
-				return status;
-			// object space output: always in the object space decode (its entry point requires parents), with parents in the others
-			if (d_inverse_bind != nullptr)
-				object_kind = k_object_skinning;
-			else if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": unknown object_kind");
-			if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
-			// plan_launch kept the poses in shared memory and gave up key frame staging first: what is left must fit one block
-			if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
-				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + composed.unfit);
-			if (num_poses == 0)
-				return ACLB200_OK;
-			params.parent_indices = d_parent_indices;
-			params.skeleton_offsets = d_skeleton_offsets;
-			params.object_flags = d_out_flags;
-			params.object_kind = object_kind;
-			params.inverse_bind = d_inverse_bind;
-			params.blend_weight = composed.weight;
-			params.blend_weights = composed.d_weights;
-			params.additive_format = composed.additive_format;
-			params.clip_additive_formats = composed.d_clip_additive_formats;
-			params.layer_masks = composed.d_layer_masks;
-			params.bone_masks = composed.d_bone_masks;
-			params.num_masks = composed.num_masks;
-			params.mask_stride = composed.mask_stride;
 			cudaSetDevice(context->device);
-			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-			const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, entry.c_str());
+			const aclb200_status cleared = clear_out_flags(context, d_out_flags, stream, what);
 			if (cleared != ACLB200_OK)
 				return cleared;
-			return finish_launch(context, launch_transform_decompress_tracks(params, composed.compose, params.db_tiers != nullptr, cuda_stream), entry.c_str());
+			return finish_launch(context, launch(), route);
 		}
 	}
 
@@ -237,14 +213,6 @@ namespace aclb200
 
 	namespace
 	{
-		// what the three skinning decodes check of their own before the composed path: parents and inverse binds
-		aclb200_status check_skinning_operands(aclb200_context* context, const uint32_t* d_parent_indices, const float* d_inverse_bind, const char* what)
-		{
-			if (d_parent_indices == nullptr)
-				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": null parent index pointer");
-			return check_inverse_binds(context, d_inverse_bind, what);
-		}
-
 		// what the two layered decodes check of their own: the stack depth, the launch's request count and the additive format
 		aclb200_status check_layers(aclb200_context* context, uint32_t num_poses, uint32_t num_layers, uint32_t additive_format, const char* what)
 		{
@@ -282,6 +250,123 @@ namespace aclb200
 			composed.num_masks = num_masks;
 			composed.mask_stride = mask_stride;
 			return ACLB200_OK;
+		}
+
+		// The composed decodes: num_poses poses of composed.num_layers requests each at d_requests. Every refusal comes before the flags are
+		// cleared: a refused call writes nothing. skinning (the _skinning entry points, which pass the matrix object kind): parents and
+		// inverse binds are required, the walk's matrices are skinned (the object kind k_object_skinning).
+		aclb200_status decompress_composed(aclb200_context* context, const aclb200_clipset* clipset, const void* d_requests, uint32_t num_poses,
+			const aclb200_options* options, const Composed& composed, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+			uint32_t object_kind, bool skinning, const float* d_inverse_bind, void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const std::string entry = composed.entry;
+			// the object space and skinning decodes require parents (the other modes take them to mean object space output), the skinning
+			// decodes inverse binds too
+			if (d_parent_indices == nullptr && (skinning || composed.compose == k_compose_object))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": null parent index pointer");
+			DecodeParams params;
+			aclb200_status status = skinning ? check_inverse_binds(context, d_inverse_bind, composed.entry) : ACLB200_OK;
+			if (status == ACLB200_OK)
+				status = make_params(context, clipset, static_cast<const aclb200_request*>(d_requests), num_poses * composed.num_layers, options, d_out,
+					true, false, params);
+			if (status == ACLB200_OK)
+				status = check_every_sub_track(context, *options, entry);
+			// object space output: always in the object space decode (its entry point requires parents), with parents in the others
+			if (status == ACLB200_OK)
+				status = check_object_output(context, *options, d_parent_indices, object_kind, entry);
+			if (status != ACLB200_OK)
+				return status;
+			// the poses stay in shared memory and give up key frame staging first: what is left must fit one block
+			params.num_layers = composed.num_layers;
+			plan_launch(params, clipset->max_key_frame_bytes, context->max_dynamic_smem, true, params.db_tiers != nullptr, composed.compose);
+			if (params.smem_bytes > uint32_t(context->max_dynamic_smem > 0 ? context->max_dynamic_smem : 0))
+				return set_error(context, ACLB200_ERR_UNSUPPORTED, entry + composed.unfit);
+			if (num_poses == 0)
+				return ACLB200_OK;
+			params.parent_indices = d_parent_indices;
+			params.skeleton_offsets = d_skeleton_offsets;
+			params.object_flags = d_out_flags;
+			params.object_kind = skinning ? k_object_skinning : object_kind;
+			params.inverse_bind = d_inverse_bind;
+			params.blend_weight = composed.weight;
+			params.blend_weights = composed.d_weights;
+			params.additive_format = composed.additive_format;
+			params.clip_additive_formats = composed.d_clip_additive_formats;
+			params.layer_masks = composed.d_layer_masks;
+			params.bone_masks = composed.d_bone_masks;
+			params.num_masks = composed.num_masks;
+			params.mask_stride = composed.mask_stride;
+			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+			return launch_clearing_flags(context, d_out_flags, cuda_stream, entry.c_str(), entry.c_str(),
+				[&] { return launch_transform_decompress_tracks(params, composed.compose, params.db_tiers != nullptr, cuda_stream); });
+		}
+
+		// Each composed decode with checks of its own and its _skinning sibling (skinning, d_inverse_bind; the matrix object kind): the checks,
+		// then the composed path
+		aclb200_status decompress_additive(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_additive_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_additive_skinning" : "decompress_tracks_additive";
+			if (num_requests > 0x7FFFFFFFu)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": more than 2^31 - 1 pairs");
+			if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": additive_format out of range");
+			// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
+			static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
+			const Composed composed = { what, k_pair_unfit, k_compose_additive, 2, 0.0f, nullptr, additive_format, d_clip_additive_formats };
+			return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
+		}
+
+		aclb200_status decompress_blend(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_blend_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, float weight, const float* d_weights,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_blend_skinning" : "decompress_tracks_blend";
+			if (num_requests > 0x7FFFFFFFu)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": more than 2^31 - 1 pairs");
+			// pair r is the two requests 2r (from) and 2r + 1 (to) of the plain decode, the layout of aclb200_additive_request
+			static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
+				"a blend request is two requests back to back");
+			const Composed composed = { what, k_pair_unfit, k_compose_blend, 2, weight, d_weights };
+			return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
+		}
+
+		aclb200_status decompress_layered(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_layer* d_layers, uint32_t num_poses,
+			uint32_t num_layers, const aclb200_options* options, uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_layered_skinning" : "decompress_tracks_layered";
+			const aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
+			if (status != ACLB200_OK)
+				return status;
+			// stack r is the requests r L .. r L + L - 1 of the launch, read as layer records by the kernel
+			static_assert(sizeof(aclb200_layer) == 16 && offsetof(aclb200_layer, pose) == 0, "a layer is a request, its op and its weight");
+			const Composed composed = { what, k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
+			return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
+		}
+
+		aclb200_status decompress_layered_masked(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_layer* d_layers,
+			const uint32_t* d_layer_masks, uint32_t num_poses, uint32_t num_layers, const float* d_bone_masks, uint32_t num_masks, uint32_t mask_stride,
+			const aclb200_options* options, uint32_t additive_format, const uint8_t* d_clip_additive_formats,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_layered_masked_skinning" : "decompress_tracks_layered_masked";
+			Composed composed = { what, k_layers_unfit, k_compose_layers_masked, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
+			aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
+			if (status == ACLB200_OK)
+				status = check_layer_masks(context, clipset, d_layer_masks, d_bone_masks, num_masks, mask_stride, what, composed);
+			if (status != ACLB200_OK)
+				return status;
+			return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
 		}
 	}
 }
@@ -451,6 +536,9 @@ extern "C"
 		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, false, params);
 		if (status != ACLB200_OK || num_requests == 0)
 			return status;
+		// launches that keep the caller's bytes store sub-tracks straight to global memory instead of assembling whole poses in shared memory
+		const bool keeps_bytes = keeps_caller_bytes(*options);
+		plan_launch(params, clipset->max_key_frame_bytes, context->max_dynamic_smem, !keeps_bytes, params.db_tiers != nullptr, k_compose_local);
 		cudaSetDevice(context->device);
 		// the plain and database kernels: one block per params.requests_per_block requests (kernels.cu, launch_tracks)
 		aclb200_launch_info& launch = context->last_launch;
@@ -468,7 +556,7 @@ extern "C"
 
 		// Main path: the persistent TMA pipeline (pipeline.cu). It assembles whole poses in shared memory, so launches that must
 		// leave `skipped` default sub-tracks untouched, or whose poses do not fit in shared memory, use the plain kernels instead.
-		if (!keeps_caller_bytes(*options) && clipset->max_key_frame_bytes != 0)
+		if (!keeps_bytes && clipset->max_key_frame_bytes != 0)
 		{
 			DecodeParams pipeline_params = params;
 			if (plan_pipeline(pipeline_params, clipset->max_key_frame_bytes, context->max_dynamic_smem, context->num_sms))
@@ -498,11 +586,9 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		if (d_parent_indices == nullptr)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_object_space: null parent index pointer");
 		const Composed composed = { "decompress_tracks_object_space", k_pose_unfit, k_compose_object, 1 };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
-			object_kind, d_out, d_out_flags, stream);
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+			false, nullptr, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -510,12 +596,9 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_skinning");
-		if (status != ACLB200_OK)
-			return status;
 		const Composed composed = { "decompress_tracks_skinning", k_pose_unfit, k_compose_object, 1 };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
-			k_object_skinning, d_out, d_out_flags, stream);
+		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets,
+			ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive(aclb200_context* context, const aclb200_clipset* clipset,
@@ -524,16 +607,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		if (num_requests > 0x7FFFFFFFu)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: more than 2^31 - 1 pairs");
-		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive: additive_format out of range");
-		// pair r is the two requests 2r (base) and 2r + 1 (additive) of the plain decode
-		static_assert(sizeof(aclb200_additive_request) == 2 * sizeof(aclb200_request), "an additive request is two requests back to back");
-		const Composed composed = { "decompress_tracks_additive", k_pair_unfit, k_compose_additive, 2, 0.0f, nullptr, additive_format,
-			d_clip_additive_formats };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
-			object_kind, d_out, d_out_flags, stream);
+		return decompress_additive(context, clipset, d_requests, num_requests, options, additive_format, d_clip_additive_formats, d_parent_indices,
+			d_skeleton_offsets, object_kind, false, nullptr, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_additive_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -542,17 +617,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		if (num_requests > 0x7FFFFFFFu)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive_skinning: more than 2^31 - 1 pairs");
-		if (additive_format > ACLB200_ADDITIVE_ADDITIVE1)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_additive_skinning: additive_format out of range");
-		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_additive_skinning");
-		if (status != ACLB200_OK)
-			return status;
-		const Composed composed = { "decompress_tracks_additive_skinning", k_pair_unfit, k_compose_additive, 2, 0.0f, nullptr, additive_format,
-			d_clip_additive_formats };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
-			k_object_skinning, d_out, d_out_flags, stream);
+		return decompress_additive(context, clipset, d_requests, num_requests, options, additive_format, d_clip_additive_formats, d_parent_indices,
+			d_skeleton_offsets, ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_apply_additive_to_base(aclb200_context* context, const void* d_base_poses, const void* d_additive_poses,
@@ -568,17 +634,13 @@ extern "C"
 		if (d_base_poses == nullptr || d_additive_poses == nullptr || d_out == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "apply_additive_to_base: null pose pointer");
 		uint64_t stride = pose_stride_bytes;
-		aclb200_status status = check_qvvf_rows(context, { d_base_poses, d_additive_poses, d_out }, num_tracks, stride, "apply_additive_to_base");
+		const aclb200_status status = check_qvvf_rows(context, { d_base_poses, d_additive_poses, d_out }, num_tracks, stride, "apply_additive_to_base");
 		if (status != ACLB200_OK)
 			return status;
-		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		status = clear_out_flags(context, d_out_flags, cuda_stream, "apply_additive_to_base");
-		if (status != ACLB200_OK)
-			return status;
-		return finish_launch(context, launch_apply_additive(static_cast<const uint8_t*>(d_base_poses), static_cast<const uint8_t*>(d_additive_poses),
-			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, additive_format, d_out_flags, context->num_sms, cuda_stream),
-			"apply_additive_to_base");
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, "apply_additive_to_base", "apply_additive_to_base", [&] {
+			return launch_apply_additive(static_cast<const uint8_t*>(d_base_poses), static_cast<const uint8_t*>(d_additive_poses),
+				static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, additive_format, d_out_flags, context->num_sms, cuda_stream); });
 	}
 
 	aclb200_status aclb200_decompress_tracks_blend(aclb200_context* context, const aclb200_clipset* clipset,
@@ -587,14 +649,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		if (num_requests > 0x7FFFFFFFu)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend: more than 2^31 - 1 pairs");
-		// pair r is the two requests 2r (from) and 2r + 1 (to) of the plain decode, the layout of aclb200_additive_request
-		static_assert(sizeof(aclb200_blend_request) == 2 * sizeof(aclb200_request) && offsetof(aclb200_blend_request, to) == sizeof(aclb200_request),
-			"a blend request is two requests back to back");
-		const Composed composed = { "decompress_tracks_blend", k_pair_unfit, k_compose_blend, 2, weight, d_weights };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, nullptr,
-			object_kind, d_out, d_out_flags, stream);
+		return decompress_blend(context, clipset, d_requests, num_requests, options, weight, d_weights, d_parent_indices, d_skeleton_offsets,
+			object_kind, false, nullptr, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_blend_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -603,14 +659,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		if (num_requests > 0x7FFFFFFFu)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "decompress_tracks_blend_skinning: more than 2^31 - 1 pairs");
-		const aclb200_status status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_blend_skinning");
-		if (status != ACLB200_OK)
-			return status;
-		const Composed composed = { "decompress_tracks_blend_skinning", k_pair_unfit, k_compose_blend, 2, weight, d_weights };
-		return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
-			k_object_skinning, d_out, d_out_flags, stream);
+		return decompress_blend(context, clipset, d_requests, num_requests, options, weight, d_weights, d_parent_indices, d_skeleton_offsets,
+			ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered(aclb200_context* context, const aclb200_clipset* clipset,
@@ -619,15 +669,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		const aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, "decompress_tracks_layered");
-		if (status != ACLB200_OK)
-			return status;
-		// stack r is the requests r L .. r L + L - 1 of the launch, read as layer records by the kernel
-		static_assert(sizeof(aclb200_layer) == 16 && offsetof(aclb200_layer, pose) == 0, "a layer is a request, its op and its weight");
-		const Composed composed = { "decompress_tracks_layered", k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format,
-			d_clip_additive_formats };
-		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, nullptr, object_kind,
-			d_out, d_out_flags, stream);
+		return decompress_layered(context, clipset, d_layers, num_poses, num_layers, options, additive_format, d_clip_additive_formats, d_parent_indices,
+			d_skeleton_offsets, object_kind, false, nullptr, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -636,15 +679,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, "decompress_tracks_layered_skinning");
-		if (status == ACLB200_OK)
-			status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, "decompress_tracks_layered_skinning");
-		if (status != ACLB200_OK)
-			return status;
-		const Composed composed = { "decompress_tracks_layered_skinning", k_layers_unfit, k_compose_layers, num_layers, 0.0f, nullptr, additive_format,
-			d_clip_additive_formats };
-		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
-			k_object_skinning, d_out, d_out_flags, stream);
+		return decompress_layered(context, clipset, d_layers, num_poses, num_layers, options, additive_format, d_clip_additive_formats, d_parent_indices,
+			d_skeleton_offsets, ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered_masked(aclb200_context* context, const aclb200_clipset* clipset,
@@ -654,15 +690,8 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		const char* what = "decompress_tracks_layered_masked";
-		Composed composed = { what, k_layers_unfit, k_compose_layers_masked, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
-		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
-		if (status == ACLB200_OK)
-			status = check_layer_masks(context, clipset, d_layer_masks, d_bone_masks, num_masks, mask_stride, what, composed);
-		if (status != ACLB200_OK)
-			return status;
-		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, nullptr, object_kind,
-			d_out, d_out_flags, stream);
+		return decompress_layered_masked(context, clipset, d_layers, d_layer_masks, num_poses, num_layers, d_bone_masks, num_masks, mask_stride, options,
+			additive_format, d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, object_kind, false, nullptr, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_tracks_layered_masked_skinning(aclb200_context* context, const aclb200_clipset* clipset,
@@ -672,17 +701,9 @@ extern "C"
 		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
-		const char* what = "decompress_tracks_layered_masked_skinning";
-		Composed composed = { what, k_layers_unfit, k_compose_layers_masked, num_layers, 0.0f, nullptr, additive_format, d_clip_additive_formats };
-		aclb200_status status = check_layers(context, num_poses, num_layers, additive_format, what);
-		if (status == ACLB200_OK)
-			status = check_layer_masks(context, clipset, d_layer_masks, d_bone_masks, num_masks, mask_stride, what, composed);
-		if (status == ACLB200_OK)
-			status = check_skinning_operands(context, d_parent_indices, d_inverse_bind, what);
-		if (status != ACLB200_OK)
-			return status;
-		return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, d_inverse_bind,
-			k_object_skinning, d_out, d_out_flags, stream);
+		return decompress_layered_masked(context, clipset, d_layers, d_layer_masks, num_poses, num_layers, d_bone_masks, num_masks, mask_stride, options,
+			additive_format, d_clip_additive_formats, d_parent_indices, d_skeleton_offsets, ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out,
+			d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_decompress_bones(aclb200_context* context, const aclb200_clipset* clipset,
@@ -696,17 +717,16 @@ extern "C"
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": bones_per_list must be 1 to 32");
 		if (num_lists == 0 || d_bone_lists == nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs at least one bone list (num_lists >= 1, d_bone_lists not NULL)");
-		// make_params refuses skip masks and `skipped` default modes for a composed decode; its pose stride check is the whole pose's, so
-		// the launch is described as a single track one and the stride of K rows is checked here
-		const Composed composed = { "decompress_bones", k_pose_unfit, k_compose_object, 1 };
+		// make_params' pose stride check is the whole pose's, so the launch is described as a single track one and the stride of K rows
+		// is checked here
 		DecodeParams params;
-		const aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, true, params, &composed);
+		aclb200_status status = make_params(context, clipset, d_requests, num_requests, options, d_out, true, true, params);
+		if (status == ACLB200_OK)
+			status = check_every_sub_track(context, *options, what);
+		if (status == ACLB200_OK)
+			status = check_object_output(context, *options, d_parent_indices, object_kind, what);
 		if (status != ACLB200_OK)
 			return status;
-		if (d_parent_indices != nullptr && object_kind != ACLB200_OBJECT_QVVF && object_kind != ACLB200_OBJECT_MATRIX3X4F)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": unknown object_kind");
-		if (d_parent_indices != nullptr && options->output_layout != ACLB200_LAYOUT_QVV48)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": object space output needs the QVV48 layout");
 		const uint64_t rows_bytes = uint64_t(bones_per_list) * params.bone_stride;
 		params.pose_stride = options->pose_stride_bytes != 0 ? options->pose_stride_bytes : rows_bytes;
 		if (params.pose_stride < rows_bytes)
@@ -725,12 +745,9 @@ extern "C"
 		query.skeleton_offsets = d_skeleton_offsets;
 		query.object_kind = object_kind;
 		query.out_flags = d_out_flags;
-		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, what.c_str());
-		if (cleared != ACLB200_OK)
-			return cleared;
-		return finish_launch(context, launch_decompress_bones(params, query, database, cuda_stream), database ? "decompress_bones (database)" : "decompress_bones");
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, what.c_str(), database ? "decompress_bones (database)" : "decompress_bones",
+			[&] { return launch_decompress_bones(params, query, database, cuda_stream); });
 	}
 
 	aclb200_status aclb200_extract_root_motion(aclb200_context* context, const aclb200_clipset* clipset,
@@ -749,27 +766,24 @@ extern "C"
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": every root sample is taken with the clamp looping policy");
 		if (options->d_request_policies != nullptr)
 			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": per request policies would override the clamp looping policy");
-		// make_params refuses skip masks and `skipped` default modes for a composed decode, a scalar clip set, NULL pointers and a misaligned
-		// output; the rows are 48 bytes apart whatever pose_stride_bytes says
+		// make_params refuses a scalar clip set, NULL pointers and a misaligned output; the rows are 48 bytes apart whatever
+		// pose_stride_bytes says
 		aclb200_options row_options = *options;
 		row_options.pose_stride_bytes = 0;
-		const Composed composed = { "extract_root_motion", k_pose_unfit, k_compose_object, 1 };
 		DecodeParams params;
-		const aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), num_requests, &row_options,
-			d_out, true, true, params, &composed);
+		aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), num_requests, &row_options, d_out,
+			true, true, params);
+		if (status == ACLB200_OK)
+			status = check_every_sub_track(context, row_options, what);
 		if (status != ACLB200_OK || num_requests == 0)
 			return status;
 		params.requests = nullptr;
 		params.pose_stride = 48;
 		const RootMotionQuery query = { d_requests, d_root_tracks, d_out_flags };
 		const bool database = params.db_tiers != nullptr;
-		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		const aclb200_status cleared = clear_out_flags(context, d_out_flags, cuda_stream, what.c_str());
-		if (cleared != ACLB200_OK)
-			return cleared;
-		return finish_launch(context, launch_extract_root_motion(params, query, database, cuda_stream),
-			database ? "extract_root_motion (database)" : "extract_root_motion");
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, what.c_str(), database ? "extract_root_motion (database)" : "extract_root_motion",
+			[&] { return launch_extract_root_motion(params, query, database, cuda_stream); });
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,
@@ -809,13 +823,10 @@ extern "C"
 		const uint32_t warps = local_to_skinning_warps(num_tracks, context->max_dynamic_smem);
 		if (warps == 0)
 			return set_error(context, ACLB200_ERR_UNSUPPORTED, "local_to_skinning: one pose does not fit in a block's shared memory");
-		cudaSetDevice(context->device);
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
-		status = clear_out_flags(context, d_out_flags, cuda_stream, "local_to_skinning");
-		if (status != ACLB200_OK)
-			return status;
-		return finish_launch(context, launch_local_to_skinning(static_cast<const uint8_t*>(d_local_poses), static_cast<uint8_t*>(d_out), num_poses,
-			num_tracks, stride, d_parent_indices, d_inverse_bind, d_out_flags, warps, context->num_sms, cuda_stream), "local_to_skinning");
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, "local_to_skinning", "local_to_skinning", [&] {
+			return launch_local_to_skinning(static_cast<const uint8_t*>(d_local_poses), static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride,
+				d_parent_indices, d_inverse_bind, d_out_flags, warps, context->num_sms, cuda_stream); });
 	}
 
 	aclb200_status aclb200_decompress_track(aclb200_context* context, const aclb200_clipset* clipset,

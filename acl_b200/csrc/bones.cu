@@ -3,8 +3,8 @@
 //
 // A request names a list of up to 32 bones. Its row j is byte for byte row list[j] of what aclb200_decompress_tracks (no parents) or
 // aclb200_decompress_tracks_object_space (parents) computes for the request: the decode is the plain kernel's decode restricted to some
-// bones (the same device decoders, SINGLE = false), and the walk is object_space.cuh's walk restricted to an ancestor-closed set of bones
-// (closure_rows_to_object_space), whose rows never read a bone outside the set.
+// bones (decode_bone_row: the plain kernel's decoders, SINGLE = false), and the walk is object_space.cuh's walk restricted to an
+// ancestor-closed set of bones (pose_rows_to_object_space<CLOSURE = true>), whose rows never read a bone outside the set.
 //
 // Work decomposition, thread block = `requests_per_block` whole requests (BoneQuery::requests_per_block):
 //   phase 1  one thread per request: the seek (seek_transform) and the request's list index, into shared memory.
@@ -12,8 +12,9 @@
 //            bitmask (max_tracks bits). It stops at a root, at a parent that does not precede its child, or at a bone another lane has
 //            already marked (that lane walks on from there). Without parents the closure is the listed bones. The warp then compacts the
 //            closure into the block's (request, bone) work list.
-//   phase 3  one thread per (request, closure bone): constant, default and animated sub-tracks of the bone, key frames read from global
-//            memory (a query touches a few sub-tracks of each key frame), into the bone's row of the request's pose rows.
+//   phase 3  one thread per (request, closure bone): decode_bone_row, the constant, default and animated sub-tracks of the bone with key
+//            frames read from global memory (a query touches a few sub-tracks of each key frame), into the bone's row of the request's
+//            pose rows.
 //   phase 4  with parents: one warp per request walks the closure bones (wavefronts of 32 bones, chunks without a closure bone skipped).
 //   phase 5  the listed rows leave shared memory as coalesced 16 byte (QVV48) or 8 byte (QVV40) stores.
 #include "device_common.cuh"
@@ -133,27 +134,8 @@ namespace aclb200
 					const uint32_t packed = s_items[item];
 					const uint32_t local_request = packed >> k_item_bone_bits;
 					const uint32_t bone = packed & ((1u << k_item_bone_bits) - 1u);
-					const RS& rs = s_req[local_request];
-					uint8_t* row = s_pose + size_t(local_request) * q.smem_pose_bytes + size_t(bone) * p.bone_stride;
-					const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
-					constant_sub_tracks<NORM, false>(p, rs, bone, desc, row);
-					if ((uint32_t(desc) & 3) == 2)
-					{
-						float rotation[4];
-						animated_rotation<NORM, PER_TRACK, false, false>(p, rs, nullptr, (uint32_t(desc) >> 2) & k_bone_index_mask, rs.alpha, rotation);
-						write_rotation(p.layout, row, rotation);
-					}
-#pragma unroll
-					for (uint32_t kind = 1; kind <= 2; ++kind)
-					{
-						const uint32_t bits = uint32_t(desc >> (k_bone_kind_shift * kind));
-						if ((bits & 3) == 2 && (kind == 1 || (rs.clip_flags & k_clip_has_scale)))
-						{
-							float value[3];
-							animated_vector<PER_TRACK, false, false>(p, rs, nullptr, kind, (bits >> 2) & k_bone_index_mask, rs.alpha, value);
-							write_vector(p.layout, row, kind, value);
-						}
-					}
+					decode_bone_row<NORM, PER_TRACK>(p, s_req[local_request], bone,
+						s_pose + size_t(local_request) * q.smem_pose_bytes + size_t(bone) * p.bone_stride);
 				}
 			}
 
@@ -168,7 +150,7 @@ namespace aclb200
 						continue;
 					const RS& rs = s_req[local_request];
 					const uint32_t skeleton = q.skeleton_offsets != nullptr ? __ldg(q.skeleton_offsets + rs.clip) : 0u;
-					flags |= obj::closure_rows_to_object_space(s_pose + size_t(local_request) * q.smem_pose_bytes, rs.num_tracks,
+					flags |= obj::pose_rows_to_object_space<true>(s_pose + size_t(local_request) * q.smem_pose_bytes, rs.num_tracks,
 						q.parent_indices + skeleton, q.object_kind != ACLB200_OBJECT_QVVF, s_mask + local_request * q.mask_words);
 				}
 				flags = __reduce_or_sync(0xFFFFFFFFu, flags);
@@ -210,17 +192,8 @@ namespace aclb200
 
 		BonesKernel bones_kernel(uint32_t normalization, bool per_track, bool database)
 		{
-			const auto pick = [&](auto norm) -> BonesKernel {
-				constexpr int NORM = decltype(norm)::value;
-				if (per_track)
-					return database ? transform_decompress_bones_kernel<NORM, true, true> : transform_decompress_bones_kernel<NORM, true, false>;
-				return database ? transform_decompress_bones_kernel<NORM, false, true> : transform_decompress_bones_kernel<NORM, false, false>;
-			};
-			if (normalization == 0)
-				return pick(std::integral_constant<int, 0>());
-			if (normalization == 1)
-				return pick(std::integral_constant<int, 1>());
-			return pick(std::integral_constant<int, 2>());
+			return with_constant<3>(normalization, [&](auto NORM) { return with_bool(per_track, [&](auto PER_TRACK) {
+				return with_bool(database, [&](auto DB) -> BonesKernel { return transform_decompress_bones_kernel<NORM, PER_TRACK, DB>; }); }); });
 		}
 	}
 

@@ -4,6 +4,8 @@
 
 #include "context.h"
 
+#include <type_traits>
+
 namespace aclb200
 {
 	namespace dev
@@ -11,6 +13,23 @@ namespace aclb200
 		constexpr uint32_t k_threads_per_block = 256;
 		constexpr uint32_t k_max_requests_per_block = 64;
 		constexpr uint32_t k_target_items_per_block = 512;
+
+		// The kernel instance of a launch from its run-time choices: f(std::integral_constant<uint32_t, value>) for a run-time value < N,
+		// f(std::bool_constant<value>) for a run-time bool; f returns the instance
+		template<uint32_t N, typename F>
+		auto with_constant(uint32_t value, F f)
+		{
+			if constexpr (N == 1)
+				return f(std::integral_constant<uint32_t, 0>());
+			else
+				return value == N - 1 ? f(std::integral_constant<uint32_t, N - 1>()) : with_constant<N - 1>(value, f);
+		}
+
+		template<typename F>
+		auto with_bool(bool value, F f)
+		{
+			return value ? f(std::true_type()) : f(std::false_type());
+		}
 
 		// ---------------------------------------------------------------------------------------------------
 		// exact float helpers
@@ -914,6 +933,34 @@ namespace aclb200
 					const float4 c = __ldg(reinterpret_cast<const float4*>(rs.image + rs.const_vec_off) + (kind == 2 ? rs.num_constant_trans : 0u) + rank);
 					v[0] = c.x; v[1] = c.y; v[2] = c.z;
 					write_vector(p.layout, out_bone, kind, v);
+				}
+			}
+		}
+
+		// One bone's row of a request for the launches that decode a few bones of each request (the bone query's closure, root motion's
+		// root): its three sub-tracks one after the other, key frames read from global memory, with the plain kernel's decoders
+		// (SINGLE = false). Those entry points refuse skip masks, so the animated sub-tracks are not checked against them: the checks made
+		// both routes 0.2 to 1 % slower (H100). decompress_track's kernel honours skip masks and keeps its own copy of this sequence.
+		template<int NORM, bool PER_TRACK, class RS>
+		__device__ __forceinline__ void decode_bone_row(const DecodeParams& p, const RS& rs, uint32_t bone, uint8_t* out_bone)
+		{
+			const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + bone);
+			constant_sub_tracks<NORM, false>(p, rs, bone, desc, out_bone);
+			if ((uint32_t(desc) & 3) == 2)
+			{
+				float rotation[4];
+				animated_rotation<NORM, PER_TRACK, false, false>(p, rs, nullptr, (uint32_t(desc) >> 2) & k_bone_index_mask, rs.alpha, rotation);
+				write_rotation(p.layout, out_bone, rotation);
+			}
+#pragma unroll
+			for (uint32_t kind = 1; kind <= 2; ++kind)
+			{
+				const uint32_t bits = uint32_t(desc >> (k_bone_kind_shift * kind));
+				if ((bits & 3) == 2 && (kind == 1 || (rs.clip_flags & k_clip_has_scale)))
+				{
+					float value[3];
+					animated_vector<PER_TRACK, false, false>(p, rs, nullptr, kind, (bits >> 2) & k_bone_index_mask, rs.alpha, value);
+					write_vector(p.layout, out_bone, kind, value);
 				}
 			}
 		}

@@ -951,22 +951,6 @@ namespace aclb200
 
 		using DecodeKernel = void (*)(DecodeParams);
 
-		// f(std::integral_constant<uint32_t, value>) for a run-time value < N, f(std::bool_constant<value>) for a run-time bool
-		template<uint32_t N, typename F>
-		DecodeKernel with_constant(uint32_t value, F f)
-		{
-			if constexpr (N == 1)
-				return f(std::integral_constant<uint32_t, 0>());
-			else
-				return value == N - 1 ? f(std::integral_constant<uint32_t, N - 1>()) : with_constant<N - 1>(value, f);
-		}
-
-		template<typename F>
-		DecodeKernel with_bool(bool value, F f)
-		{
-			return value ? f(std::true_type()) : f(std::false_type());
-		}
-
 		// The transform_decompress_tracks_kernel instance of a launch, nullptr for a choice no plan makes: a composed decode always assembles
 		// its poses in shared memory. configure_kernels walks every choice through here, so every kernel a launch can pick is configured.
 		DecodeKernel tracks_kernel(uint32_t normalization, bool per_track, bool database, bool staged, bool out_staged, uint32_t compose)

@@ -1,5 +1,6 @@
 // acl_b200/csrc/object_space.cuh -- the hierarchy walk shared by the error measurement (error_metric.cu: object_space_kernel), the object
-// space decode (kernels.cu: transform_decompress_tracks_kernel<..., COMPOSE = k_compose_object>) and the bone query (bones.cu): the reference's
+// space decode (kernels.cu: transform_decompress_tracks_kernel<..., COMPOSE = k_compose_object>) and the bone query (bones.cu, the walk
+// restricted to the ancestor closure of the listed bones): the reference's
 // qvv and 3x4 matrix operations in unfused IEEE operations, and the wavefront loop one warp runs over a pose. Also acl::apply_additive_to_base, which
 // the error measurement, the additive decode (COMPOSE = k_compose_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which
 // the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share. And the skinning step, which the three composed decodes (with
@@ -489,15 +490,29 @@ namespace aclb200
 			// qvvf_transform_error_metric::local_to_object_space (transform_error_metrics.h:289-310) or, MATRIX, convert_transforms +
 			// local_to_object_space of qvvf_matrix3x4f_transform_error_metric (:397-436). Every lane of the warp calls it; returns the lane's
 			// ACLB200_ERROR_FLAG_* bits.
-			__device__ __forceinline__ uint32_t pose_rows_to_object_space(uint8_t* pose, uint32_t num_tracks, const uint32_t* parents, bool matrix)
+			// CLOSURE (the bone query): only the bones of `closure` (bit b % 32 of word b / 32: bone b; no bit at or above num_tracks), an
+			// ancestor-closed set: the parent of a closure bone is in the closure, unless it does not precede the bone (then the bone is a
+			// root, as in the whole walk). The same row operations and wavefronts on the closure bones only, chunks of 32 bones without one
+			// skipped: a closure row ends byte for byte as the whole walk leaves it, and no other row is read or written. A template
+			// argument rather than a run-time mask, so that the whole walk's code carries no mask.
+			template<bool CLOSURE = false>
+			__device__ __forceinline__ uint32_t pose_rows_to_object_space(uint8_t* pose, uint32_t num_tracks, const uint32_t* parents, bool matrix,
+				const uint32_t* closure = nullptr)
 			{
 				const Fp<float> fp{};
 				const uint32_t lane = threadIdx.x & 31u;
 				uint32_t flags = 0;
 				for (uint32_t base = 0; base < num_tracks; base += 32)
 				{
+					uint32_t word = 0;
+					if (CLOSURE)
+					{
+						word = closure[base >> 5];
+						if (word == 0)
+							continue;
+					}
 					const uint32_t bone = base + lane;
-					const bool active = bone < num_tracks;
+					const bool active = CLOSURE ? ((word >> lane) & 1u) != 0 : bone < num_tracks;
 					uint32_t parent = active ? __ldg(parents + bone) : k_invalid_track;
 					if (parent_follows(active, bone, parent))
 					{
@@ -531,67 +546,6 @@ namespace aclb200
 							else
 							{
 								// rtm::qvv_normalize(rtm::qvv_mul(local, parent_object)), qvvf.h:426-430
-								Qvv<float> object = qvv_mul_positive(fp, mine, up);
-								object.rotation = quat_normalize(fp, object.rotation);
-								store_qvv_row(row, object);
-							}
-						});
-					}
-				}
-				return flags;
-			}
-
-			// pose_rows_to_object_space restricted to the bones of `closure` (bit b % 32 of word b / 32: bone b; no bit at or above
-			// num_tracks), an ancestor-closed set: the parent of a closure bone is in the closure, unless it does not precede the bone (then
-			// the bone is a root, as in the whole walk). The same row operations and wavefronts on the closure bones only, chunks of 32 bones
-			// without one skipped: a closure row ends byte for byte as pose_rows_to_object_space leaves it, and no other row is read or
-			// written. Its own copy of the loop, so that the whole walk's code is not touched by the mask. Every lane of the warp calls it;
-			// returns the lane's ACLB200_ERROR_FLAG_* bits (of closure bones only).
-			__device__ __forceinline__ uint32_t closure_rows_to_object_space(uint8_t* pose, uint32_t num_tracks, const uint32_t* parents, bool matrix,
-				const uint32_t* closure)
-			{
-				const Fp<float> fp{};
-				const uint32_t lane = threadIdx.x & 31u;
-				uint32_t flags = 0;
-				for (uint32_t base = 0; base < num_tracks; base += 32)
-				{
-					const uint32_t word = closure[base >> 5];
-					if (word == 0)
-						continue;
-					const uint32_t bone = base + lane;
-					const bool active = ((word >> lane) & 1u) != 0;
-					uint32_t parent = active ? __ldg(parents + bone) : k_invalid_track;
-					if (parent_follows(active, bone, parent))
-					{
-						flags |= ACLB200_ERROR_FLAG_INVALID_SKELETON;
-						parent = k_invalid_track;
-					}
-					float4* row = reinterpret_cast<float4*>(pose + size_t(bone) * 48);
-					if (matrix)
-					{
-						if (active)
-							store_matrix_row(row, matrix_from_qvv(fp, load_qvv_row(row)));		// convert_transforms
-						__syncwarp();
-						wavefront_walk(active, parent, base, [&]()
-						{
-							const float4* above = reinterpret_cast<const float4*>(pose + size_t(parent) * 48);
-							store_matrix_row(row, matrix_mul(fp, load_matrix_row(row), load_matrix_row(above)));
-						});
-					}
-					else
-					{
-						wavefront_walk(active, parent, base, [&]()
-						{
-							const float4* above = reinterpret_cast<const float4*>(pose + size_t(parent) * 48);
-							const Qvv<float> mine = load_qvv_row(row);
-							const Qvv<float> up = load_qvv_row(above);
-							if (takes_negative_branch(fp, mine.scale, up.scale))
-							{
-								flags |= ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
-								object_row_slow(row, above);
-							}
-							else
-							{
 								Qvv<float> object = qvv_mul_positive(fp, mine, up);
 								object.rotation = quat_normalize(fp, object.rotation);
 								store_qvv_row(row, object);

@@ -2,9 +2,8 @@
 // request, across loop boundaries, composed from root samples taken with the clamp policy.
 //
 // A request needs up to four samples of its clip's root track: T(from), T(to) and, when playback crossed a loop boundary, the clip's two
-// ends T(D) and T(0). Each sample is the root's row of aclb200_decompress_tracks for {clip, t}: the same seek (seek_request) and the same
-// device decoders with SINGLE = false (constant_sub_tracks, animated_rotation, animated_vector), restricted to one bone as the bone query
-// restricts them to its closure (bones.cu phase 3).
+// ends T(D) and T(0). Each sample is the root's row of aclb200_decompress_tracks for {clip, t}: the same seek (seek_request) and the bone
+// decoder the bone query runs on its closure (decode_bone_row: the plain kernel's decoders, SINGLE = false), for the root only.
 //
 // Work decomposition, thread block = 64 requests, one lane per (request, sample slot), 8 requests per warp:
 //   slot 0 from_time, slot 1 to_time, slot 2 the clamp duration D, slot 3 time 0. The lane seeks its own time and decodes the root's three
@@ -95,26 +94,7 @@ namespace aclb200
 				seek_request<DB>(p, aclb200_request{ clip_index, time }, uint32_t(request_index), rs);
 				// the decoders write through a pointer, but at constant offsets of `row` once inlined: the row stays in registers (the kernel's
 				// local memory is only the argument block of the out-of-line negative scale path, obj::qvv_mul_negative_scale)
-				uint8_t* bone = reinterpret_cast<uint8_t*>(row);
-				const uint64_t desc = __ldg(reinterpret_cast<const unsigned long long*>(rs.image + rs.bone_table_off) + root);
-				constant_sub_tracks<NORM, false>(p, rs, root, desc, bone);
-				if ((uint32_t(desc) & 3) == 2)
-				{
-					float rotation[4];
-					animated_rotation<NORM, PER_TRACK, false, false>(p, rs, nullptr, (uint32_t(desc) >> 2) & k_bone_index_mask, rs.alpha, rotation);
-					write_rotation(p.layout, bone, rotation);
-				}
-#pragma unroll
-				for (uint32_t kind = 1; kind <= 2; ++kind)
-				{
-					const uint32_t bits = uint32_t(desc >> (k_bone_kind_shift * kind));
-					if ((bits & 3) == 2 && (kind == 1 || (rs.clip_flags & k_clip_has_scale)))
-					{
-						float value[3];
-						animated_vector<PER_TRACK, false, false>(p, rs, nullptr, kind, (bits >> 2) & k_bone_index_mask, rs.alpha, value);
-						write_vector(p.layout, bone, kind, value);
-					}
-				}
+				decode_bone_row<NORM, PER_TRACK>(p, rs, root, reinterpret_cast<uint8_t*>(row));
 			}
 
 			// ---- the request's slot 0 lane composes M from the four samples ----
@@ -155,17 +135,8 @@ namespace aclb200
 
 		RootMotionKernel root_motion_kernel(uint32_t normalization, bool per_track, bool database)
 		{
-			const auto pick = [&](auto norm) -> RootMotionKernel {
-				constexpr int NORM = decltype(norm)::value;
-				if (per_track)
-					return database ? extract_root_motion_kernel<NORM, true, true> : extract_root_motion_kernel<NORM, true, false>;
-				return database ? extract_root_motion_kernel<NORM, false, true> : extract_root_motion_kernel<NORM, false, false>;
-			};
-			if (normalization == 0)
-				return pick(std::integral_constant<int, 0>());
-			if (normalization == 1)
-				return pick(std::integral_constant<int, 1>());
-			return pick(std::integral_constant<int, 2>());
+			return with_constant<3>(normalization, [&](auto NORM) { return with_bool(per_track, [&](auto PER_TRACK) {
+				return with_bool(database, [&](auto DB) -> RootMotionKernel { return extract_root_motion_kernel<NORM, PER_TRACK, DB>; }); }); });
 		}
 	}
 
