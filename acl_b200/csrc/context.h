@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../include/aclb200.h"
+#include "base_pose_cache.h"
 #include "layout.h"
 
 struct aclb200_context
@@ -46,24 +47,13 @@ struct aclb200_context
 
 namespace aclb200
 {
-	// What a clip's base pose row (constant + default sub-tracks in the output layout, pipeline.cu) depends on besides the clip
-	struct BasePoseKey
-	{
-		uint32_t layout;
-		uint32_t normalize_always;
-		uint32_t default_mode[3];
-		float    constant_defaults[12];
-	};
-
+	// One cached base pose variant of a clip set (pipeline.cu); its key and pins are kept by BasePoseCache (base_pose_cache.h)
 	struct BasePoseRows
 	{
-		BasePoseKey key;
 		uint8_t* d_rows = nullptr;			// [num_clips][row_stride]
 		uint32_t row_stride = 0;
 		cudaEvent_t ready = nullptr;		// recorded after the build kernel on the stream that asked for it first
-		cudaEvent_t last_launch = nullptr;	// recorded after the latest launch that reads the rows
-		uint32_t users = 0;					// launches being set up with these rows (between acquire and release)
-		uint64_t last_use = 0;
+		cudaEvent_t last_launch = nullptr;	// recorded after the latest launch that reads the rows, on that launch's stream
 	};
 }
 
@@ -87,10 +77,10 @@ struct aclb200_clipset
 	std::vector<uint32_t> host_blob_db_offset;		// [num_clips] clip_header_offset of its tracks_database_header, 0xFFFFFFFF without one
 	std::vector<std::vector<uint32_t>> host_db_pose_bits;	// animated_pose_bit_size of each segment of the clips bound to a database
 
-	// base pose rows built on first use per (layout, normalisation, default modes, default values), a handful kept
+	// base pose rows built on first use per (layout, normalisation, default modes, constant default values), a handful kept, under
+	// base_mutex
 	mutable std::mutex base_mutex;
-	mutable std::vector<aclb200::BasePoseRows> base_rows;
-	mutable uint64_t base_clock = 0;
+	mutable aclb200::BasePoseCache<aclb200::BasePoseRows> base_poses;
 };
 
 // A compressed_database on the device (database.cpp): the blob's headers stay on the host, the tier metadata and the streamed in
