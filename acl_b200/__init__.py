@@ -20,4 +20,5 @@ from .api import (  # noqa: F401
     LAYER_OFF, LAYER_BLEND, LAYER_ADDITIVE, LAYER_NO_MASK, MAX_LAYERS, LAYER_DTYPE, make_layers,
     NO_BONE, MAX_QUERY_BONES,
     MAX_ROOT_MOTION_CYCLES, ROOT_MOTION_REQUEST_DTYPE, make_root_motion_requests,
+    FEATURE_CLAMP, FEATURE_LOOP, MAX_FEATURE_OFFSETS, FEATURE_REQUEST_DTYPE, make_feature_requests,
 )

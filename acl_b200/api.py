@@ -175,6 +175,7 @@ def _lib():
                                                                         vp, vp, vp, vp, vp]
         l.aclb200_decompress_bones.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, u32, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_extract_root_motion.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, vp, vp]
+        l.aclb200_extract_pose_features.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -206,7 +207,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
         "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
-        "aclb200_extract_root_motion",
+        "aclb200_extract_root_motion", "aclb200_extract_pose_features",
     ]
 
 
@@ -257,6 +258,10 @@ LAYER_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("op",
 MAX_ROOT_MOTION_CYCLES = 256     # the most loop boundaries one extract_root_motion request may cross
 # numpy view of aclb200_root_motion_request {uint32 clip; float from_time; float to_time; int32 cycles}
 ROOT_MOTION_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("from_time", np.float32), ("to_time", np.float32), ("cycles", np.int32)])
+FEATURE_CLAMP, FEATURE_LOOP = 0, 1   # extract_pose_features: an offset time beyond the clip's ends is clamped, or wraps into another cycle
+MAX_FEATURE_OFFSETS = 8          # the most time offsets of one extract_pose_features launch
+# numpy view of aclb200_feature_request {uint32 clip; float time; uint32 looping}
+FEATURE_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("time", np.float32), ("looping", np.uint32)])
 
 
 def make_layers(clips, times, ops, weights) -> np.ndarray:
@@ -282,6 +287,18 @@ def make_root_motion_requests(clips, from_times, to_times, cycles=0) -> np.ndarr
     out["from_time"] = from_times
     out["to_time"] = to_times
     out["cycles"] = cycles
+    return out.reshape(-1)
+
+
+def make_feature_requests(clips, times, looping=FEATURE_CLAMP) -> np.ndarray:
+    """(clip index, current playback time, FEATURE_CLAMP / FEATURE_LOOP) arrays, or anything that broadcasts to one shape ->
+    aclb200_feature_request[]"""
+    clips, times, looping = np.broadcast_arrays(np.asarray(clips, dtype=np.uint32), np.asarray(times, dtype=np.float32),
+                                                np.asarray(looping, dtype=np.uint32))
+    out = np.empty(clips.shape, dtype=FEATURE_REQUEST_DTYPE)
+    out["clip"] = clips
+    out["time"] = times
+    out["looping"] = looping
     return out.reshape(-1)
 
 
@@ -550,6 +567,23 @@ class Context:
         self._check(_lib().aclb200_extract_root_motion(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
                                                        _device_ptr(d_root_tracks), _device_ptr(d_out), _device_ptr(d_out_flags),
                                                        _stream_ptr(stream)))
+
+    def extract_pose_features(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, offsets, d_bone_lists,
+                              bones_per_list: int, d_parent_indices, d_out, num_lists: int = 1, d_request_lists=None, d_root_tracks=None,
+                              d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """Pose features of num_requests make_feature_requests at each time offset of `offsets` (host floats, seconds, 1..8 of them): row
+        (s, k) of request r at d_out + r * pose_stride + (s * K + k) * 48 (pose_stride: options.pose_stride_bytes, 0 = S * K rows) is
+        qvv_mul(qvv_mul(B, qvv_inverse(T)), M), the object row B of bone list[k] at u' = t + offsets[s] (wrapped into the clip under
+        FEATURE_LOOP) carried into the root's frame at t: T is the root's local row at u', M root motion from t to u'. Bone lists as
+        decompress_bones; the root of clip c is d_root_tracks[c] (uint32, None: track 0); clip c's skeleton is d_parent_indices +
+        d_skeleton_offsets[c]. options need the QVV48 layout and LOOP_CLAMP. d_out_flags: optional uint32 ERROR_FLAG_* of the walk, of M
+        and of the rows."""
+        values = np.ascontiguousarray(offsets, dtype=np.float32).reshape(-1)
+        self._check(_lib().aclb200_extract_pose_features(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
+                                                         values.ctypes.data if values.size else None, values.size,
+                                                         _device_ptr(d_bone_lists), num_lists, bones_per_list, _device_ptr(d_request_lists),
+                                                         _device_ptr(d_root_tracks), _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                         _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as

@@ -1,6 +1,7 @@
 // acl_b200/csrc/api.cpp -- the extern "C" surface declared in include/aclb200.h.
 #include "context.h"
 
+#include <cmath>
 #include <cstddef>
 #include <cstring>
 #include <functional>
@@ -162,6 +163,29 @@ namespace aclb200
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": unknown object_kind");
 			if (d_parent_indices != nullptr && options.output_layout != ACLB200_LAYOUT_QVV48)
 				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": object space output needs the QVV48 layout");
+			return ACLB200_OK;
+		}
+
+		// the bone lists of the bone query and the pose features: K = bones_per_list of 1..32 entries, at least one list
+		aclb200_status check_bone_lists(aclb200_context* context, const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list,
+			const std::string& entry)
+		{
+			if (bones_per_list == 0 || bones_per_list > ACLB200_MAX_QUERY_BONES)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": bones_per_list must be 1 to 32");
+			if (num_lists == 0 || d_bone_lists == nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": needs at least one bone list (num_lists >= 1, d_bone_lists not NULL)");
+			return ACLB200_OK;
+		}
+
+		// the root samples of root motion and the pose features: QVV48 rows, every one taken with the clamp looping policy
+		aclb200_status check_root_samples(aclb200_context* context, const aclb200_options& options, const std::string& entry)
+		{
+			if (options.output_layout != ACLB200_LAYOUT_QVV48)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": the root samples and the output are QVV48 rows");
+			if (options.looping_policy != ACLB200_LOOP_CLAMP)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": every root sample is taken with the clamp looping policy");
+			if (options.d_request_policies != nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, entry + ": per request policies would override the clamp looping policy");
 			return ACLB200_OK;
 		}
 
@@ -377,7 +401,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.13 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.14 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -438,7 +462,7 @@ extern "C"
 		context->num_sms = prop.multiProcessorCount;
 		context->max_dynamic_smem = int(prop.sharedMemPerBlockOptin);
 		if (prop.major != 9 || prop.minor != 0 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess
-			|| configure_bones_kernels(context->max_dynamic_smem) != cudaSuccess)
+			|| configure_bones_kernels(context->max_dynamic_smem) != cudaSuccess || configure_features_kernels(context->max_dynamic_smem) != cudaSuccess)
 		{
 			// the kernels are compiled for sm_90a only, which runs on compute capability 9.0 and nothing else
 			delete context;
@@ -713,10 +737,9 @@ extern "C"
 		void* d_out, uint32_t* d_out_flags, void* stream)
 	{
 		const std::string what = "decompress_bones";
-		if (bones_per_list == 0 || bones_per_list > ACLB200_MAX_QUERY_BONES)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": bones_per_list must be 1 to 32");
-		if (num_lists == 0 || d_bone_lists == nullptr)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs at least one bone list (num_lists >= 1, d_bone_lists not NULL)");
+		const aclb200_status lists_checked = check_bone_lists(context, d_bone_lists, num_lists, bones_per_list, what);
+		if (lists_checked != ACLB200_OK)
+			return lists_checked;
 		// make_params' pose stride check is the whole pose's, so the launch is described as a single track one and the stride of K rows
 		// is checked here
 		DecodeParams params;
@@ -760,12 +783,9 @@ extern "C"
 		const aclb200_status checked = check_handles_and_options(context, clipset, options);
 		if (checked != ACLB200_OK)
 			return checked;
-		if (options->output_layout != ACLB200_LAYOUT_QVV48)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": the root samples and the output are QVV48 rows");
-		if (options->looping_policy != ACLB200_LOOP_CLAMP)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": every root sample is taken with the clamp looping policy");
-		if (options->d_request_policies != nullptr)
-			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": per request policies would override the clamp looping policy");
+		const aclb200_status samples_checked = check_root_samples(context, *options, what);
+		if (samples_checked != ACLB200_OK)
+			return samples_checked;
 		// make_params refuses a scalar clip set, NULL pointers and a misaligned output; the rows are 48 bytes apart whatever
 		// pose_stride_bytes says
 		aclb200_options row_options = *options;
@@ -784,6 +804,74 @@ extern "C"
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 		return launch_clearing_flags(context, d_out_flags, cuda_stream, what.c_str(), database ? "extract_root_motion (database)" : "extract_root_motion",
 			[&] { return launch_extract_root_motion(params, query, database, cuda_stream); });
+	}
+
+	aclb200_status aclb200_extract_pose_features(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_feature_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const float* offsets, uint32_t num_offsets,
+		const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
+		const uint32_t* d_root_tracks, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		static_assert(sizeof(aclb200_feature_request) == 12, "a feature request is three 4 byte fields");
+		const std::string what = "extract_pose_features";
+		// the handles and the options struct's size before any option is read
+		const aclb200_status checked = check_handles_and_options(context, clipset, options);
+		if (checked != ACLB200_OK)
+			return checked;
+		if (offsets == nullptr || num_offsets == 0 || num_offsets > ACLB200_MAX_FEATURE_OFFSETS)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs 1 to 8 offsets (num_offsets), offsets not NULL");
+		for (uint32_t s = 0; s < num_offsets; ++s)
+			if (!std::isfinite(offsets[s]))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": every offset must be finite");
+		if (uint64_t(num_requests) * num_offsets > 0xFFFFFFFFull)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": num_requests * num_offsets must fit in 32 bits");
+		if (d_parent_indices == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": the features are object space rows, d_parent_indices must be given");
+		const aclb200_status lists_checked = check_bone_lists(context, d_bone_lists, num_lists, bones_per_list, what);
+		if (lists_checked != ACLB200_OK)
+			return lists_checked;
+		const aclb200_status samples_checked = check_root_samples(context, *options, what);
+		if (samples_checked != ACLB200_OK)
+			return samples_checked;
+		// make_params refuses a scalar clip set, NULL pointers and a misaligned output; the stride of S * K rows is checked here
+		DecodeParams params;
+		aclb200_status status = make_params(context, clipset, reinterpret_cast<const aclb200_request*>(d_requests), num_requests, options, d_out,
+			true, true, params);
+		if (status == ACLB200_OK)
+			status = check_every_sub_track(context, *options, what);
+		if (status == ACLB200_OK)
+			status = check_object_output(context, *options, d_parent_indices, ACLB200_OBJECT_QVVF, what);
+		if (status != ACLB200_OK)
+			return status;
+		const uint64_t rows_bytes = uint64_t(num_offsets) * bones_per_list * 48;
+		params.pose_stride = options->pose_stride_bytes != 0 ? options->pose_stride_bytes : rows_bytes;
+		if (params.pose_stride < rows_bytes)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": pose_stride_bytes is smaller than num_offsets * bones_per_list rows");
+		const bool database = params.db_tiers != nullptr;
+		BoneQuery query = {};
+		if (!plan_features_launch(params, query, database, context->max_dynamic_smem))
+			return set_error(context, ACLB200_ERR_UNSUPPORTED, what + k_pose_unfit);
+		if (num_requests == 0)
+			return ACLB200_OK;
+		params.requests = nullptr;
+		params.num_requests = num_requests * num_offsets;
+		query.bone_lists = d_bone_lists;
+		query.request_lists = d_request_lists;
+		query.num_lists = num_lists;
+		query.bones_per_list = bones_per_list;
+		query.parent_indices = d_parent_indices;
+		query.skeleton_offsets = d_skeleton_offsets;
+		query.object_kind = ACLB200_OBJECT_QVVF;
+		query.out_flags = d_out_flags;
+		FeatureQuery features = {};
+		features.requests = d_requests;
+		features.root_tracks = d_root_tracks;
+		std::memcpy(features.offsets, offsets, num_offsets * sizeof(float));
+		features.num_offsets = num_offsets;
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, what.c_str(), database ? "extract_pose_features (database)" : "extract_pose_features",
+			[&] { return launch_extract_pose_features(params, query, features, database, cuda_stream); });
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

@@ -7,18 +7,11 @@
 // ancestor-closed set of bones (pose_rows_to_object_space<CLOSURE = true>), whose rows never read a bone outside the set.
 //
 // Work decomposition, thread block = `requests_per_block` whole requests (BoneQuery::requests_per_block):
+//   bone_query_block (bone_closure.cuh, shared with the pose features) with BoneRowsStage:
 //   phase 1  one thread per request: the seek (seek_transform) and the request's list index, into shared memory.
-//   phase 2  one warp per request, one lane per list entry: the lane walks its bone's parents and ORs them into the request's closure
-//            bitmask (max_tracks bits). It stops at a root, at a parent that does not precede its child, or at a bone another lane has
-//            already marked (that lane walks on from there). Without parents the closure is the listed bones. The warp then compacts the
-//            closure into the block's (request, bone) work list.
-//   phase 3  one thread per (request, closure bone): decode_bone_row, the constant, default and animated sub-tracks of the bone with key
-//            frames read from global memory (a query touches a few sub-tracks of each key frame), into the bone's row of the request's
-//            pose rows.
-//   phase 4  with parents: one warp per request walks the closure bones (wavefronts of 32 bones, chunks without a closure bone skipped).
+//   phases 2 to 4  each request's ancestor closure is marked, listed, decoded (decode_bone_row) and, with parents, walked to object space.
 //   phase 5  the listed rows leave shared memory as coalesced 16 byte (QVV48) or 8 byte (QVV40) stores.
-#include "device_common.cuh"
-#include "object_space.cuh"
+#include "bone_closure.cuh"
 
 #include <type_traits>
 
@@ -30,34 +23,14 @@ namespace aclb200
 	{
 		constexpr uint32_t k_bones_target_requests = 8;				// one request per warp of the walk
 		constexpr uint32_t k_bones_block_budget = 48u * 1024u;		// up to 4 blocks of 8 C2 requests per SM
-		constexpr uint32_t k_item_bone_bits = 26;					// a work item: bone | local request << 26 (64 requests, 2^26 bones)
-		static_assert(k_max_tracks <= (1u << k_item_bone_bits) && k_max_requests_per_block <= 64, "a work item holds a bone and a request");
 
-		// per request words beside the request states: [0] the list index (k_no_list: the request writes nothing), [1] the first work item
-		// of the request, [2] its closure size
-		constexpr uint32_t k_no_list = 0xFFFFFFFFu;
-
-		template<int NORM, bool PER_TRACK, bool DB>
-		__global__ void __launch_bounds__(k_threads_per_block)
-		transform_decompress_bones_kernel(const DecodeParams p, const BoneQuery q)
+		// phase 1 and phase 5 of the bone query's block (bone_closure.cuh)
+		template<bool DB>
+		struct BoneRowsStage
 		{
-			using RS = typename std::conditional<DB, ReqStateDB, ReqState>::type;
-			// dynamic shared memory: RS[requests_per_block] | request words u32[requests_per_block][4] | closure bitmasks
-			// u32[requests_per_block][mask_words] | work items u32[requests_per_block * max_tracks] | pose rows
-			extern __shared__ __align__(16) uint8_t s_dynamic[];
-			RS* s_req = reinterpret_cast<RS*>(s_dynamic);
-			uint32_t* s_words = reinterpret_cast<uint32_t*>(s_dynamic + q.smem_words_offset);
-			uint32_t* s_mask = reinterpret_cast<uint32_t*>(s_dynamic + q.smem_mask_offset);
-			uint32_t* s_items = reinterpret_cast<uint32_t*>(s_dynamic + q.smem_items_offset);
-			uint8_t* s_pose = s_dynamic + q.smem_pose_offset;
-
-			const uint32_t first_request = blockIdx.x * q.requests_per_block;
-			const uint32_t num_requests = min(q.requests_per_block, p.num_requests - first_request);
-			const uint32_t lane = threadIdx.x & 31u;
-			const uint32_t warp = threadIdx.x >> 5;
-
-			// ---- phase 1: seek, list index; the closure bitmasks are cleared ----
-			if (threadIdx.x < num_requests)
+			// ---- phase 1: the seek (seek_transform) and the request's list index; a list index >= num_lists writes nothing ----
+			template<class RS>
+			__device__ __forceinline__ void seek(const DecodeParams& p, const BoneQuery& q, uint32_t first_request, RS* s_req, uint32_t* s_words) const
 			{
 				RS rs;
 				seek_transform<DB>(p, first_request + threadIdx.x, rs);
@@ -67,100 +40,16 @@ namespace aclb200
 				s_req[threadIdx.x] = rs;
 				s_words[threadIdx.x * 4] = rs.num_tracks != 0 ? list : k_no_list;
 			}
-			for (uint32_t word = threadIdx.x; word < num_requests * q.mask_words; word += k_threads_per_block)
-				s_mask[word] = 0;
-			__syncthreads();
 
-			// ---- phase 2: one warp per request marks the ancestor closure of its listed bones, counts it ----
-			for (uint32_t local_request = warp; local_request < num_requests; local_request += k_threads_per_block / 32)
-			{
-				const uint32_t list = s_words[local_request * 4];
-				uint32_t* mask = s_mask + local_request * q.mask_words;
-				uint32_t count = 0;
-				if (list != k_no_list)
-				{
-					const uint32_t num_tracks = s_req[local_request].num_tracks;
-					const uint32_t* parents = nullptr;
-					if (q.parent_indices != nullptr)
-						parents = q.parent_indices + (q.skeleton_offsets != nullptr ? __ldg(q.skeleton_offsets + s_req[local_request].clip) : 0u);
-					uint32_t bone = lane < q.bones_per_list ? __ldg(q.bone_lists + size_t(list) * q.bones_per_list + lane) : obj::k_invalid_track;
-					// a walk only ever moves to a parent strictly below its bone: it ends on any parent table
-					while (bone < num_tracks)
-					{
-						const uint32_t bit = 1u << (bone & 31u);
-						if ((atomicOr(mask + (bone >> 5), bit) & bit) != 0 || parents == nullptr)
-							break;
-						const uint32_t parent = __ldg(parents + bone);
-						bone = parent < bone ? parent : obj::k_invalid_track;
-					}
-					__syncwarp();
-					for (uint32_t word = lane; word < q.mask_words; word += 32)
-						count += __popc(mask[word]);
-					count = __reduce_add_sync(0xFFFFFFFFu, count);
-				}
-				if (lane == 0)
-					s_words[local_request * 4 + 2] = count;
-			}
-			__syncthreads();
-
-			// ---- the work list: request r's closure bones at items [first of r, first of r + count of r), in bone order ----
-			for (uint32_t local_request = warp; local_request < num_requests; local_request += k_threads_per_block / 32)
-			{
-				uint32_t first = 0;
-				for (uint32_t r = lane; r < local_request; r += 32)
-					first += s_words[r * 4 + 2];
-				first = __reduce_add_sync(0xFFFFFFFFu, first);
-				if (lane == 0)
-					s_words[local_request * 4 + 1] = first;
-				if (s_words[local_request * 4 + 2] == 0)
-					continue;
-				const uint32_t* mask = s_mask + local_request * q.mask_words;
-				for (uint32_t word_index = 0; word_index < q.mask_words; ++word_index)
-				{
-					const uint32_t word = mask[word_index];
-					if (((word >> lane) & 1u) != 0)
-						s_items[first + __popc(word & ((1u << lane) - 1u))] = (word_index * 32 + lane) | (local_request << k_item_bone_bits);
-					first += __popc(word);
-				}
-			}
-			__syncthreads();
-
-			// ---- phase 3: one thread per (request, closure bone) decodes the bone's three sub-tracks into its row ----
-			{
-				const uint32_t last = num_requests - 1;
-				const uint32_t num_items = s_words[last * 4 + 1] + s_words[last * 4 + 2];
-				for (uint32_t item = threadIdx.x; item < num_items; item += k_threads_per_block)
-				{
-					const uint32_t packed = s_items[item];
-					const uint32_t local_request = packed >> k_item_bone_bits;
-					const uint32_t bone = packed & ((1u << k_item_bone_bits) - 1u);
-					decode_bone_row<NORM, PER_TRACK>(p, s_req[local_request], bone,
-						s_pose + size_t(local_request) * q.smem_pose_bytes + size_t(bone) * p.bone_stride);
-				}
-			}
-
-			// ---- phase 4: one warp per request takes its closure rows to object space ----
-			if (q.parent_indices != nullptr)
-			{
-				__syncthreads();
-				uint32_t flags = 0;
-				for (uint32_t local_request = warp; local_request < num_requests; local_request += k_threads_per_block / 32)
-				{
-					if (s_words[local_request * 4 + 2] == 0)
-						continue;
-					const RS& rs = s_req[local_request];
-					const uint32_t skeleton = q.skeleton_offsets != nullptr ? __ldg(q.skeleton_offsets + rs.clip) : 0u;
-					flags |= obj::pose_rows_to_object_space<true>(s_pose + size_t(local_request) * q.smem_pose_bytes, rs.num_tracks,
-						q.parent_indices + skeleton, q.object_kind != ACLB200_OBJECT_QVVF, s_mask + local_request * q.mask_words);
-				}
-				flags = __reduce_or_sync(0xFFFFFFFFu, flags);
-				if (lane == 0 && flags != 0 && q.out_flags != nullptr)
-					atomicOr(q.out_flags, flags);
-			}
+			template<class RS>
+			__device__ __forceinline__ void before_closures(const DecodeParams&, const RS*, const uint32_t*, uint32_t, uint32_t) const {}
 
 			// ---- phase 5: row j of request r is row list[j] of its pose rows; 16 byte chunks (QVV48) or 8 byte chunks (QVV40) ----
-			__syncthreads();
+			template<class RS>
+			__device__ __forceinline__ void finish(const DecodeParams& p, const BoneQuery& q, const RS* s_req, const uint32_t* s_words,
+				const uint8_t* s_pose, uint32_t first_request, uint32_t num_requests) const
 			{
+				__syncthreads();
 				const bool qvv40 = p.layout == ACLB200_LAYOUT_QVV40;
 				const uint32_t chunk_bytes = qvv40 ? 8u : 16u;
 				const uint32_t chunks_per_row = p.bone_stride / chunk_bytes;
@@ -186,6 +75,13 @@ namespace aclb200
 						*reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
 				}
 			}
+		};
+
+		template<int NORM, bool PER_TRACK, bool DB>
+		__global__ void __launch_bounds__(k_threads_per_block)
+		transform_decompress_bones_kernel(const DecodeParams p, const BoneQuery q)
+		{
+			bone_query_block<NORM, PER_TRACK, DB>(p, q, BoneRowsStage<DB>{});
 		}
 
 		using BonesKernel = void (*)(DecodeParams, BoneQuery);
@@ -208,7 +104,7 @@ namespace aclb200
 
 	// Up to 8 requests per block within 48 KB, at least one within the whole budget: max_tracks pose rows per request, as the object space
 	// decode plans them, plus the closure bitmask, the request's share of the work list and its state
-	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem)
+	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem, uint32_t extra_request_bytes)
 	{
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t state_bytes = database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState));
@@ -221,7 +117,7 @@ namespace aclb200
 			query.smem_mask_offset = (query.smem_words_offset + requests * 16 + 15) & ~15u;
 			query.smem_items_offset = query.smem_mask_offset + requests * query.mask_words * 4;
 			query.smem_pose_offset = (query.smem_items_offset + requests * max_tracks * 4 + 15) & ~15u;
-			const uint64_t bytes = query.smem_pose_offset + uint64_t(requests) * query.smem_pose_bytes;
+			const uint64_t bytes = query.smem_pose_offset + uint64_t(requests) * (uint64_t(query.smem_pose_bytes) + extra_request_bytes);
 			query.smem_bytes = uint32_t(bytes < 0xFFFFFFFFu ? bytes : 0xFFFFFFFFu);
 			return bytes;
 		};

@@ -229,6 +229,17 @@ namespace aclb200
 		uint32_t* out_flags;					// ACLB200_ERROR_FLAG_NEGATIVE_SCALE and ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE are OR-ed in, or nullptr
 	};
 
+	// The pose features (aclb200_extract_pose_features, features.cu): a third kernel argument beside DecodeParams and the bone query's
+	// BoneQuery. The launch runs the bone query's plan on virtual requests r * num_offsets + s (request r at offset s): DecodeParams'
+	// num_requests counts them and its `requests` is unused.
+	struct FeatureQuery
+	{
+		const aclb200_feature_request* requests;
+		const uint32_t* root_tracks;			// [num_clips] the root track of each clip, or nullptr (track 0)
+		float offsets[ACLB200_MAX_FEATURE_OFFSETS];
+		uint32_t num_offsets;					// S, 1..ACLB200_MAX_FEATURE_OFFSETS
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
@@ -270,12 +281,18 @@ namespace aclb200
 	cudaError_t launch_scalar_decompress_tracks(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t launch_scalar_decompress_track(const DecodeParams& params, cudaStream_t stream);
 	cudaError_t configure_kernels(int& max_dynamic_smem);
-	// bones.cu: the bone query. plan_bones_launch returns false when one request does not fit max_dynamic_smem.
+	// bones.cu: the bone query. plan_bones_launch returns false when one request does not fit max_dynamic_smem; `extra_request_bytes`
+	// (16 byte granular) per request follow the pose rows (the pose features' root samples).
 	cudaError_t configure_bones_kernels(int max_dynamic_smem);
-	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem);
+	bool plan_bones_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem, uint32_t extra_request_bytes = 0);
 	cudaError_t launch_decompress_bones(const DecodeParams& params, const BoneQuery& query, bool database, cudaStream_t stream);
 	// root_motion.cu: root motion, one lane per (request, sample)
 	cudaError_t launch_extract_root_motion(const DecodeParams& params, const RootMotionQuery& query, bool database, cudaStream_t stream);
+	// features.cu: the pose features, on the bone query's plan (plan_features_launch: false when one pose does not fit max_dynamic_smem)
+	cudaError_t configure_features_kernels(int max_dynamic_smem);
+	bool plan_features_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem);
+	cudaError_t launch_extract_pose_features(const DecodeParams& params, const BoneQuery& query, const FeatureQuery& features, bool database,
+		cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

@@ -5,7 +5,7 @@
 // the error measurement, the additive decode (COMPOSE = k_compose_additive) and aclb200_apply_additive_to_base share, and rtm::qvv_lerp, which
 // the blend decode (COMPOSE = k_compose_blend) and aclb200_blend_poses share. And the skinning step, which the three composed decodes (with
 // the internal object kind k_object_skinning) and aclb200_local_to_skinning run after the matrix walk. And rtm::qvv_inverse, which root motion
-// (root_motion.cu) composes with qvv_mul.
+// (root_motion.cu) composes with qvv_mul, and root motion's composition for the pose features (features.cu).
 //
 // The wavefront loop: a warp takes 32 consecutive bones at a time; a lane whose parent lies in an earlier chunk -- or was finished by an
 // earlier wavefront of this chunk -- computes, the others wait for the next wavefront (skeletons are shallow and bushy: a handful of
@@ -401,6 +401,41 @@ namespace aclb200
 				const Vec3<float> rotated = quat_mul_vector3(fp, scaled, out.rotation);
 				out.translation = Vec3<float>{ neg(rotated.x), neg(rotated.y), neg(rotated.z) };
 				return out;
+			}
+
+			// rtm::qvv_mul(lhs, rhs) through whichever branch it takes; the matrix branch (a mirrored operand) is reported
+			__device__ __forceinline__ Qvv<float> flagged_qvv_mul(const Qvv<float>& lhs, const Qvv<float>& rhs, uint32_t& flags)
+			{
+				if (takes_negative_branch(Fp<float>{}, lhs.scale, rhs.scale))
+					flags |= ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
+				return qvv_mul_any(lhs, rhs);
+			}
+
+			// M of aclb200_extract_root_motion from the root samples T(from), T(to), T(D) (end) and T(0) (start), |cycles| <= 256: root
+			// motion (root_motion.cu) composes it per request, the pose features (features.cu) per (request, offset). `clip_flags` is the
+			// clip's ClipDesc::flags: a loop crossing on a clip compressed with the wrap policy is reported.
+			__device__ __forceinline__ Qvv<float> compose_root_motion(const Qvv<float>& from, const Qvv<float>& to, const Qvv<float>& end,
+				const Qvv<float>& start, int32_t cycles, uint32_t clip_flags, uint32_t& flags)
+			{
+				Qvv<float> motion;
+				if (cycles == 0)
+					motion = flagged_qvv_mul(to, qvv_inverse(from), flags);		// rel(from, to)
+				else
+				{
+					// forward: the boundary reached is the end, playback resumes at the start; backward the other way round
+					const bool forward = cycles > 0;
+					const Qvv<float> reached = forward ? end : start;
+					const Qvv<float> inverse_resumed = qvv_inverse(forward ? start : end);
+					motion = flagged_qvv_mul(reached, qvv_inverse(from), flags);				// rel(from, reached)
+					const Qvv<float> cycle = flagged_qvv_mul(reached, inverse_resumed, flags);		// rel(resumed, reached), once
+					const int32_t full_cycles = (forward ? cycles : -cycles) - 1;
+					for (int32_t i = 0; i < full_cycles; ++i)
+						motion = flagged_qvv_mul(cycle, motion, flags);
+					motion = flagged_qvv_mul(flagged_qvv_mul(to, inverse_resumed, flags), motion, flags);	// rel(resumed, to)
+					if (clip_flags & k_clip_wrap)
+						flags |= ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE;
+				}
+				return motion;
 			}
 
 			// planes[bone] = qvv_normalize(qvv_mul(planes[bone] (the local transform), planes[parent])), every stream

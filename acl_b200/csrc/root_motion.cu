@@ -8,8 +8,9 @@
 // Work decomposition, thread block = 64 requests, one lane per (request, sample slot), 8 requests per warp:
 //   slot 0 from_time, slot 1 to_time, slot 2 the clamp duration D, slot 3 time 0. The lane seeks its own time and decodes the root's three
 //   sub-tracks into a row in registers; the cycle end slots decode nothing when the request crosses no boundary.
-//   The request's slot 0 lane gathers the other three rows with __shfl_sync, composes M (rtm::qvv_inverse, rtm::qvv_mul in unfused IEEE
-//   operations, object_space.cuh) and stores its 48 byte row. No pose row goes through shared memory.
+//   The request's slot 0 lane gathers the other three rows with __shfl_sync, composes M (obj::compose_root_motion: rtm::qvv_inverse,
+//   rtm::qvv_mul in unfused IEEE operations, object_space.cuh, shared with the pose features) and stores its 48 byte row. No pose row
+//   goes through shared memory.
 #include "device_common.cuh"
 #include "object_space.cuh"
 
@@ -28,14 +29,6 @@ namespace aclb200
 		using obj::Qvv;
 		using obj::Quat;
 		using obj::Vec3;
-
-		// rtm::qvv_mul(lhs, rhs) through whichever branch it takes; the matrix branch (a mirrored root) is reported
-		__device__ __forceinline__ Qvv<float> qvv_mul_flagged(const Qvv<float>& lhs, const Qvv<float>& rhs, uint32_t& flags)
-		{
-			if (obj::takes_negative_branch(obj::Fp<float>{}, lhs.scale, rhs.scale))
-				flags |= ACLB200_ERROR_FLAG_NEGATIVE_SCALE;
-			return obj::qvv_mul_any(lhs, rhs);
-		}
 
 		// the row of lane `source` of the warp, as an rtm::qvvf
 		__device__ __forceinline__ Qvv<float> shuffle_row(const float4 row[3], uint32_t source)
@@ -105,27 +98,8 @@ namespace aclb200
 			const Qvv<float> start = shuffle_row(row, first + 3);
 			uint32_t flags = 0;
 			if (slot == 0 && writes)
-			{
-				Qvv<float> motion;
-				if (cycles == 0)
-					motion = qvv_mul_flagged(to, obj::qvv_inverse(from), flags);		// rel(from, to)
-				else
-				{
-					// forward: the boundary reached is the end, playback resumes at the start; backward the other way round
-					const bool forward = cycles > 0;
-					const Qvv<float> reached = forward ? end : start;
-					const Qvv<float> inverse_resumed = obj::qvv_inverse(forward ? start : end);
-					motion = qvv_mul_flagged(reached, obj::qvv_inverse(from), flags);				// rel(from, reached)
-					const Qvv<float> cycle = qvv_mul_flagged(reached, inverse_resumed, flags);		// rel(resumed, reached), once
-					const int32_t full_cycles = (forward ? cycles : -cycles) - 1;
-					for (int32_t i = 0; i < full_cycles; ++i)
-						motion = qvv_mul_flagged(cycle, motion, flags);
-					motion = qvv_mul_flagged(qvv_mul_flagged(to, inverse_resumed, flags), motion, flags);	// rel(resumed, to)
-					if (clip_flags & k_clip_wrap)
-						flags |= ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE;
-				}
-				obj::store_qvv_row(reinterpret_cast<float4*>(p.out + request_index * 48), motion);
-			}
+				obj::store_qvv_row(reinterpret_cast<float4*>(p.out + request_index * 48),
+					obj::compose_root_motion(from, to, end, start, cycles, clip_flags, flags));
 			flags = __reduce_or_sync(0xFFFFFFFFu, flags);
 			if (lane == 0 && flags != 0 && q.out_flags != nullptr)
 				atomicOr(q.out_flags, flags);

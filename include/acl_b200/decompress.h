@@ -536,6 +536,19 @@ namespace acl_b200
 			m_device->check(aclb200_extract_root_motion(m_device->get(), m_clipset, d_requests, num_requests, &options, d_root_tracks, d_out, d_out_flags,
 				stream), "aclb200_extract_root_motion");
 		}
+		// Pose features (aclb200_extract_pose_features): for each request and each of the num_offsets host `offsets` (seconds, 1..8), the
+		// object rows of its bone list's bones at t + offset (wrapped into the clip for ACLB200_FEATURE_LOOP requests) in the root's frame at
+		// t, row (s, k) of request r at d_out + r * pose_stride + (s * bones_per_list + k) * 48. The root of clip c is d_root_tracks[c]
+		// (nullptr: track 0), its skeleton d_parent_indices + d_skeleton_offsets[c]. options need the QVV48 layout and ACLB200_LOOP_CLAMP.
+		void extract_pose_features(const aclb200_feature_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const float* offsets, uint32_t num_offsets, const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list,
+			const uint32_t* d_parent_indices, void* d_out, const uint32_t* d_request_lists = nullptr, const uint32_t* d_root_tracks = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_extract_pose_features(m_device->get(), m_clipset, d_requests, num_requests, &options, offsets, num_offsets,
+				d_bone_lists, num_lists, bones_per_list, d_request_lists, d_root_tracks, d_parent_indices, d_skeleton_offsets, d_out, d_out_flags,
+				stream), "aclb200_extract_pose_features");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

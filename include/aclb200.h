@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 13
+#define ACLB200_VERSION_MINOR 14
 
 typedef enum aclb200_status
 {
@@ -728,6 +728,60 @@ typedef struct aclb200_root_motion_request
 ACLB200_API aclb200_status aclb200_extract_root_motion(aclb200_context* context, const aclb200_clipset* clipset,
 	const aclb200_root_motion_request* d_requests, uint32_t num_requests, const aclb200_options* options,
 	const uint32_t* d_root_tracks, void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* One pose features request: the playback time of a character on one clip, and how its offsets reach beyond the clip's ends */
+typedef struct aclb200_feature_request
+{
+	uint32_t clip;				/* index into the clip set */
+	float    time;				/* the current playback time t, seconds */
+	uint32_t looping;			/* ACLB200_FEATURE_CLAMP or ACLB200_FEATURE_LOOP */
+} aclb200_feature_request;
+
+/* aclb200_feature_request::looping: an offset time beyond the clip's ends is clamped, or wraps around into the next or previous cycle */
+#define ACLB200_FEATURE_CLAMP 0u
+#define ACLB200_FEATURE_LOOP 1u
+/* The most time offsets of one aclb200_extract_pose_features launch */
+#define ACLB200_MAX_FEATURE_OFFSETS 8
+
+/* Pose features (motion matching): chosen bones of each request at up to eight time offsets, each in the character's frame at the request's
+ * time, in one launch. For request r, offset s (S = num_offsets) and entry k of the request's bone list (K = bones_per_list):
+ *   d_requests      device aclb200_feature_request[num_requests] (12 bytes each), 4 byte aligned.
+ *   offsets         HOST float[num_offsets] in seconds (1..ACLB200_MAX_FEATURE_OFFSETS), copied into the launch: negative for the past, 0
+ *                   for the current pose, positive for the predicted trajectory.
+ *   bone lists      as aclb200_decompress_bones (d_bone_lists, num_lists, bones_per_list, d_request_lists).
+ *   root track      d_root_tracks[clip] (device uint32[num_clips]), or track 0 when d_root_tracks is NULL. D is the clip's clamp duration,
+ *                   as aclb200_extract_root_motion's.
+ *   offset time     u = t + offsets[s] (one IEEE single add). ACLB200_FEATURE_CLAMP: c = 0, u' = u (the seek clamps u' as
+ *                   aclb200_decompress_tracks does). ACLB200_FEATURE_LOOP: D == 0 gives c = 0, u' = 0; otherwise c = (int32) floorf(u / D)
+ *                   and u' = u - float(c) * D, an IEEE divide, multiply and subtract, none fused.
+ *   M_s             byte for byte the row aclb200_extract_root_motion writes for {clip, t, u', c} with the same options and root.
+ *   T_s             the root track's local row at u': aclb200_decompress_tracks's QVV48 row with the clamp policy.
+ *   B_{s,k}         byte for byte row list[k] of aclb200_decompress_bones with the same parents and ACLB200_OBJECT_QVVF for {clip, u'}.
+ *   row             F = rtm::qvv_mul(rtm::qvv_mul(B, rtm::qvv_inverse(T_s)), M_s), both branches of qvv_mul: the bone at time t + offsets[s]
+ *                   in the root's frame at time t. When the root track is a root of the skeleton, its own entry is M_s up to rounding (the
+ *                   trajectory). Velocities are differences of two offsets' translations.
+ *   d_out           row (s, k) of request r at d_out + r * pose_stride + (s * K + k) * 48, 48 byte rows of the ACLB200_OBJECT_QVVF layout, 16
+ *                   byte aligned; pose_stride = options->pose_stride_bytes, 0 = S * K * 48.
+ *   untouched       every row of a request with an invalid clip index, a list index >= num_lists, a root at or beyond its clip's num_tracks
+ *                   or a looping value other than 0 and 1; the K rows of an offset whose u is not finite under ACLB200_FEATURE_LOOP or whose
+ *                   |c| > ACLB200_MAX_ROOT_MOTION_CYCLES; the row of an entry that is ACLB200_NO_BONE or at or beyond its clip's num_tracks.
+ *   d_out_flags     device uint32, optional: cleared, then OR-ed in: ACLB200_ERROR_FLAG_NEGATIVE_SCALE when a qvv_mul of the walk, of M or of
+ *                   F took its matrix branch; ACLB200_ERROR_FLAG_INVALID_SKELETON from the walk; ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE when an
+ *                   offset that writes its rows has c != 0 on a clip compressed with the wrap policy (as aclb200_extract_root_motion).
+ * As aclb200_decompress_bones and aclb200_extract_root_motion: a bound database's streamed tiers are read, variable defaults and the batch
+ * and per track rounding policies are honoured, ACLB200_MATH_FAST is accepted and runs the exact decode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing and leaving *d_out_flags untouched: NULL offsets, a non-finite offset,
+ * num_offsets 0 or above ACLB200_MAX_FEATURE_OFFSETS, num_requests * num_offsets above 2^32 - 1, NULL d_parent_indices, the bone list
+ * refusals of aclb200_decompress_bones, the refusals of aclb200_extract_root_motion (output_layout other than QVV48, looping_policy other
+ * than ACLB200_LOOP_CLAMP, d_request_policies, skip masks or a `skipped` default mode, a scalar clip set), NULL d_requests or d_out with
+ * num_requests > 0, a pose stride below S * K * 48, rows not 16 byte aligned. ACLB200_ERR_UNSUPPORTED when one pose of the widest clip does
+ * not fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_extract_pose_features(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_feature_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const float* offsets, uint32_t num_offsets,
+	const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
+	const uint32_t* d_root_tracks, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
+	void* d_out, uint32_t* d_out_flags, void* stream);
 
 /* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
  * aclb200_apply_additive_to_base): num_poses poses of rtm::qvvf rows of one skeleton (48 byte bones, 16 byte aligned, pose p at
