@@ -21,4 +21,6 @@ from .api import (  # noqa: F401
     NO_BONE, MAX_QUERY_BONES,
     MAX_ROOT_MOTION_CYCLES, ROOT_MOTION_REQUEST_DTYPE, make_root_motion_requests,
     FEATURE_CLAMP, FEATURE_LOOP, MAX_FEATURE_OFFSETS, FEATURE_REQUEST_DTYPE, make_feature_requests,
+    FEATURE_POSITION, FEATURE_DIRECTION, FEATURE_VELOCITY, MAX_FEATURE_DIMS, NO_ROW, FEATURE_TERM_DTYPE, SEARCH_QUERY_DTYPE,
+    SEARCH_RESULT_DTYPE, make_feature_terms, feature_term_dims, make_search_queries,
 )

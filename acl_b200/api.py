@@ -176,6 +176,8 @@ def _lib():
         l.aclb200_decompress_bones.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, u32, vp, vp, vp, u32, vp, vp, vp]
         l.aclb200_extract_root_motion.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, vp, vp, vp]
         l.aclb200_extract_pose_features.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]
+        l.aclb200_pack_pose_features.argtypes = [vp, vp, u32, u32, u32, u64, vp, u32, vp, vp, u32, vp, u32, vp]
+        l.aclb200_search_pose_features.argtypes = [vp, vp, u64, u64, vp, vp, vp, u32, u64, u32, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -207,7 +209,7 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_additive_skinning", "aclb200_decompress_tracks_blend_skinning", "aclb200_local_to_skinning",
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
         "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
-        "aclb200_extract_root_motion", "aclb200_extract_pose_features",
+        "aclb200_extract_root_motion", "aclb200_extract_pose_features", "aclb200_pack_pose_features", "aclb200_search_pose_features",
     ]
 
 
@@ -262,6 +264,14 @@ FEATURE_CLAMP, FEATURE_LOOP = 0, 1   # extract_pose_features: an offset time bey
 MAX_FEATURE_OFFSETS = 8          # the most time offsets of one extract_pose_features launch
 # numpy view of aclb200_feature_request {uint32 clip; float time; uint32 looping}
 FEATURE_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("time", np.float32), ("looping", np.uint32)])
+FEATURE_POSITION, FEATURE_DIRECTION, FEATURE_VELOCITY = 0, 1, 2   # pack_pose_features term kinds
+MAX_FEATURE_DIMS = 64            # the most dimensions of a packed feature vector
+NO_ROW = 0xFFFFFFFF              # search_pose_features: the row of a query without a candidate
+# numpy views of aclb200_feature_term, aclb200_search_query and aclb200_search_result
+FEATURE_TERM_DTYPE = np.dtype([("kind", np.uint32), ("s0", np.uint32), ("s1", np.uint32), ("k", np.uint32), ("axis", np.uint32),
+                               ("components", np.uint32), ("inv_dt", np.float32)])
+SEARCH_QUERY_DTYPE = np.dtype([("tag_mask", np.uint32), ("exclude_begin", np.uint32), ("exclude_end", np.uint32)])
+SEARCH_RESULT_DTYPE = np.dtype([("row", np.uint32), ("cost", np.float32)])
 
 
 def make_layers(clips, times, ops, weights) -> np.ndarray:
@@ -299,6 +309,34 @@ def make_feature_requests(clips, times, looping=FEATURE_CLAMP) -> np.ndarray:
     out["clip"] = clips
     out["time"] = times
     out["looping"] = looping
+    return out.reshape(-1)
+
+
+def make_feature_terms(kinds, s0, k, components=7, s1=0, axis=0, inv_dt=0.0) -> np.ndarray:
+    """(FEATURE_* kind, offset s0, bone list entry k, x = 1 | y = 2 | z = 4 component mask, later offset s1 of a velocity, axis of a
+    direction, 1 / dt of a velocity) arrays, or anything that broadcasts to one shape -> aclb200_feature_term[]"""
+    fields = np.broadcast_arrays(np.asarray(kinds, dtype=np.uint32), np.asarray(s0, dtype=np.uint32), np.asarray(s1, dtype=np.uint32),
+                                 np.asarray(k, dtype=np.uint32), np.asarray(axis, dtype=np.uint32), np.asarray(components, dtype=np.uint32),
+                                 np.asarray(inv_dt, dtype=np.float32))
+    out = np.empty(fields[0].shape, dtype=FEATURE_TERM_DTYPE)
+    for name, value in zip(FEATURE_TERM_DTYPE.names, fields):
+        out[name] = value
+    return out.reshape(-1)
+
+
+def feature_term_dims(terms: np.ndarray) -> int:
+    """D of a term array: the number of components its masks emit"""
+    return int(sum(bin(int(c) & 7).count("1") for c in np.asarray(terms)["components"]))
+
+
+def make_search_queries(tag_masks=0xFFFFFFFF, exclude_begin=0, exclude_end=0) -> np.ndarray:
+    """(tag mask, first excluded row, end of the excluded rows) arrays, or anything that broadcasts to one shape -> aclb200_search_query[]"""
+    masks, begin, end = np.broadcast_arrays(np.asarray(tag_masks, dtype=np.uint32), np.asarray(exclude_begin, dtype=np.uint32),
+                                            np.asarray(exclude_end, dtype=np.uint32))
+    out = np.empty(masks.shape, dtype=SEARCH_QUERY_DTYPE)
+    out["tag_mask"] = masks
+    out["exclude_begin"] = begin
+    out["exclude_end"] = end
     return out.reshape(-1)
 
 
@@ -584,6 +622,32 @@ class Context:
                                                          _device_ptr(d_bone_lists), num_lists, bones_per_list, _device_ptr(d_request_lists),
                                                          _device_ptr(d_root_tracks), _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
                                                          _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def pack_pose_features(self, d_rows, num_requests: int, num_offsets: int, bones_per_list: int, terms: np.ndarray, d_out, out_stride: int,
+                           mean=None, scale=None, pose_stride_bytes: int = 0, num_dims: int | None = None, stream=None) -> None:
+        """Feature vectors of num_requests requests' extract_pose_features rows (S = num_offsets, K = bones_per_list, pose_stride_bytes 0 =
+        S * K rows): the terms (make_feature_terms, host) emit their components in order, out[r][d] = (v_d - mean[d]) * scale[d] (host
+        float32 arrays, None: 0 and 1) at d_out + r * out_stride floats. num_dims defaults to the terms' component count."""
+        terms = np.ascontiguousarray(terms, dtype=FEATURE_TERM_DTYPE).reshape(-1)
+        dims = feature_term_dims(terms) if num_dims is None else num_dims
+        stats = [None if a is None else np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in (mean, scale)]
+        for a in stats:
+            if a is not None and a.size < dims:
+                raise ValueError("mean and scale need one float per dimension")
+        self._check(_lib().aclb200_pack_pose_features(self._handle, _device_ptr(d_rows), num_requests, num_offsets, bones_per_list,
+                                                      pose_stride_bytes, terms.ctypes.data if terms.size else None, terms.size,
+                                                      *[None if a is None else a.ctypes.data for a in stats], dims, _device_ptr(d_out),
+                                                      out_stride, _stream_ptr(stream)))
+
+    def search_pose_features(self, d_database, num_rows: int, db_stride: int, d_query_vectors, d_queries, num_queries: int, q_stride: int,
+                             num_dims: int, d_results, d_row_tags=None, stream=None) -> None:
+        """The best row of each query: d_results[q] (SEARCH_RESULT_DTYPE, 8 bytes) = the allowed row with the lowest cost
+        sum_d fmaf(q[d] - x[d], ...) (the lowest row on a tie; {NO_ROW, +inf} without one). Row r is allowed for query q
+        (make_search_queries) when it is outside [exclude_begin, exclude_end), d_row_tags[r] & tag_mask != 0 (uint32, None: every tag set)
+        and its cost is not NaN. Strides are in floats."""
+        self._check(_lib().aclb200_search_pose_features(self._handle, _device_ptr(d_database), num_rows, db_stride, _device_ptr(d_row_tags),
+                                                        _device_ptr(d_query_vectors), _device_ptr(d_queries), num_queries, q_stride, num_dims,
+                                                        _device_ptr(d_results), _stream_ptr(stream)))
 
     # ---- skinning matrices: the matrix walk, then rtm::matrix_mul(inverse_bind, object) per bone. d_inverse_bind holds 12 floats per
     # skeleton entry (x_axis, y_axis, z_axis, w_axis, xyz each), 16 byte aligned, in parallel with d_parent_indices. Each bone leaves as

@@ -401,7 +401,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.14 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.15 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -462,7 +462,8 @@ extern "C"
 		context->num_sms = prop.multiProcessorCount;
 		context->max_dynamic_smem = int(prop.sharedMemPerBlockOptin);
 		if (prop.major != 9 || prop.minor != 0 || cudaSetDevice(device) != cudaSuccess || configure_kernels(context->max_dynamic_smem) != cudaSuccess
-			|| configure_bones_kernels(context->max_dynamic_smem) != cudaSuccess || configure_features_kernels(context->max_dynamic_smem) != cudaSuccess)
+			|| configure_bones_kernels(context->max_dynamic_smem) != cudaSuccess || configure_features_kernels(context->max_dynamic_smem) != cudaSuccess
+			|| configure_feature_search_kernels() != cudaSuccess)
 		{
 			// the kernels are compiled for sm_90a only, which runs on compute capability 9.0 and nothing else
 			delete context;
@@ -872,6 +873,114 @@ extern "C"
 		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 		return launch_clearing_flags(context, d_out_flags, cuda_stream, what.c_str(), database ? "extract_pose_features (database)" : "extract_pose_features",
 			[&] { return launch_extract_pose_features(params, query, features, database, cuda_stream); });
+	}
+
+	aclb200_status aclb200_pack_pose_features(aclb200_context* context, const void* d_rows, uint32_t num_requests, uint32_t num_offsets,
+		uint32_t bones_per_list, uint64_t pose_stride_bytes, const aclb200_feature_term* terms, uint32_t num_terms, const float* mean,
+		const float* scale, uint32_t num_dims, float* d_out, uint32_t out_stride, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		const std::string what = "pack_pose_features";
+		if (num_offsets == 0 || num_offsets > ACLB200_MAX_FEATURE_OFFSETS || bones_per_list == 0 || bones_per_list > ACLB200_MAX_QUERY_BONES)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs 1 to 8 offsets and 1 to 32 bones per list");
+		if (num_dims == 0 || num_dims > ACLB200_MAX_FEATURE_DIMS)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": num_dims must be 1 to 64");
+		if (terms == nullptr || num_terms == 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": needs at least one term");
+		PackParams params = {};
+		uint32_t d = 0;
+		for (uint32_t t = 0; t < num_terms; ++t)
+		{
+			const aclb200_feature_term& term = terms[t];
+			if (term.kind > ACLB200_FEATURE_VELOCITY || term.s0 >= num_offsets || term.k >= bones_per_list || term.components == 0
+				|| term.components > 7 || (term.kind == ACLB200_FEATURE_VELOCITY && (term.s1 >= num_offsets || !std::isfinite(term.inv_dt)))
+				|| (term.kind == ACLB200_FEATURE_DIRECTION && term.axis > 2))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": term " + std::to_string(t)
+					+ " has an unknown kind, a row outside the S x K rows, an axis above 2, components outside 1..7 or a non-finite inv_dt");
+			for (uint32_t c = 0; c < 3; ++c)
+			{
+				if ((term.components & (1u << c)) == 0)
+					continue;
+				if (d == num_dims)
+					return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": the terms emit more than num_dims components");
+				PackDim& dim = params.dims[d];
+				dim.kind = term.kind;
+				dim.row0 = term.s0 * bones_per_list + term.k;
+				dim.row1 = term.kind == ACLB200_FEATURE_VELOCITY ? term.s1 * bones_per_list + term.k : dim.row0;
+				dim.component = c;
+				dim.axis = term.kind == ACLB200_FEATURE_DIRECTION ? term.axis : 0u;
+				dim.inv_dt = term.kind == ACLB200_FEATURE_VELOCITY ? term.inv_dt : 1.0f;
+				dim.mean = mean != nullptr ? mean[d] : 0.0f;
+				dim.scale = scale != nullptr ? scale[d] : 1.0f;
+				if (!std::isfinite(dim.mean) || !std::isfinite(dim.scale))
+					return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": mean and scale must be finite");
+				++d;
+			}
+		}
+		if (d != num_dims)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": the terms emit fewer than num_dims components");
+		const uint64_t rows_bytes = uint64_t(num_offsets) * bones_per_list * 48;
+		const uint64_t pose_stride = pose_stride_bytes != 0 ? pose_stride_bytes : rows_bytes;
+		if (pose_stride < rows_bytes || (pose_stride % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": pose_stride_bytes must hold S * K rows and be a multiple of 16");
+		if (out_stride < num_dims || (out_stride % 4) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": out_stride must be at least num_dims and a multiple of 4 floats");
+		if (num_requests == 0)
+			return ACLB200_OK;
+		if (d_rows == nullptr || d_out == nullptr || ((reinterpret_cast<uintptr_t>(d_rows) | reinterpret_cast<uintptr_t>(d_out)) % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": d_rows and d_out must be 16 byte aligned device pointers");
+		params.rows = static_cast<const uint8_t*>(d_rows);
+		params.pose_stride = pose_stride;
+		params.out = d_out;
+		params.out_stride = out_stride;
+		params.num_requests = num_requests;
+		params.num_dims = num_dims;
+		cudaSetDevice(context->device);
+		return finish_launch(context, launch_pack_pose_features(params, static_cast<cudaStream_t>(stream)), what.c_str());
+	}
+
+	aclb200_status aclb200_search_pose_features(aclb200_context* context, const float* d_database, uint64_t num_rows, uint64_t db_stride,
+		const uint32_t* d_row_tags, const float* d_query_vectors, const aclb200_search_query* d_queries, uint32_t num_queries, uint64_t q_stride,
+		uint32_t num_dims, aclb200_search_result* d_results, void* stream)
+	{
+		static_assert(sizeof(aclb200_search_result) == 8 && offsetof(aclb200_search_result, cost) == 4,
+			"a result read as a little endian uint64 is (cost bits << 32) | row");
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		const std::string what = "search_pose_features";
+		if (num_dims == 0 || num_dims > ACLB200_MAX_FEATURE_DIMS)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": num_dims must be 1 to 64");
+		if (db_stride < num_dims || q_stride < num_dims || (db_stride % 4) != 0 || (q_stride % 4) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": db_stride and q_stride must be at least num_dims and multiples of 4 floats");
+		if (num_rows >= 0xFFFFFFFFull)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": num_rows must be below 2^32 - 1 (ACLB200_NO_ROW)");
+		if (num_rows != 0 && d_database == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": null database");
+		if (num_queries != 0 && (d_query_vectors == nullptr || d_queries == nullptr || d_results == nullptr))
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": null query / result pointer");
+		if (((reinterpret_cast<uintptr_t>(d_database) | reinterpret_cast<uintptr_t>(d_query_vectors)) % 16) != 0
+			|| (reinterpret_cast<uintptr_t>(d_results) % 8) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, what + ": vectors must be 16 byte aligned, results 8 byte aligned");
+		if (num_queries == 0)
+			return ACLB200_OK;
+		SearchParams params = {};
+		params.database = d_database;
+		params.query_vectors = d_query_vectors;
+		params.queries = d_queries;
+		params.row_tags = d_row_tags;
+		params.results = d_results;
+		params.num_rows = num_rows;
+		params.db_stride = db_stride;
+		params.q_stride = q_stride;
+		params.num_queries = num_queries;
+		params.num_dims = num_dims;
+		cudaSetDevice(context->device);
+		const aclb200_status status = finish_launch(context, launch_search_pose_features(params, context->num_sms, static_cast<cudaStream_t>(stream)),
+			what.c_str());
+		if (status == ACLB200_OK && num_rows != 0)
+			context->launch_count++;		// the results' clear, then the search: two kernels
+		return status;
 	}
 
 	aclb200_status aclb200_blend_poses(aclb200_context* context, const void* d_from_poses, const void* d_to_poses, void* d_out,

@@ -240,6 +240,44 @@ namespace aclb200
 		uint32_t num_offsets;					// S, 1..ACLB200_MAX_FEATURE_OFFSETS
 	};
 
+	// The pack (aclb200_pack_pose_features, feature_search.cu): each output dimension resolved from its term on the host
+	struct PackDim
+	{
+		uint32_t kind;							// ACLB200_FEATURE_POSITION / DIRECTION / VELOCITY
+		uint32_t row0;							// s0 * K + k: the row read (VELOCITY: subtracted)
+		uint32_t row1;							// VELOCITY: s1 * K + k
+		uint32_t component;						// 0, 1, 2 = x, y, z
+		uint32_t axis;							// DIRECTION: the unit axis rotated
+		float inv_dt;							// VELOCITY
+		float mean;
+		float scale;
+	};
+	struct PackParams
+	{
+		const uint8_t* rows;					// request r's rows at rows + r * pose_stride, 48 bytes each
+		uint64_t pose_stride;
+		float* out;								// request r's vector at out + r * out_stride
+		uint64_t out_stride;					// floats
+		uint32_t num_requests;
+		uint32_t num_dims;
+		PackDim dims[ACLB200_MAX_FEATURE_DIMS];
+	};
+
+	// The search (aclb200_search_pose_features, feature_search.cu)
+	struct SearchParams
+	{
+		const float* database;					// row r at database + r * db_stride
+		const float* query_vectors;				// query q at query_vectors + q * q_stride
+		const aclb200_search_query* queries;
+		const uint32_t* row_tags;				// [num_rows], or nullptr (every tag 0xFFFFFFFF)
+		aclb200_search_result* results;
+		uint64_t num_rows;						// N < 2^32 - 1
+		uint64_t db_stride;						// floats
+		uint64_t q_stride;
+		uint32_t num_queries;
+		uint32_t num_dims;
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
@@ -293,6 +331,10 @@ namespace aclb200
 	bool plan_features_launch(const DecodeParams& params, BoneQuery& query, bool database, int max_dynamic_smem);
 	cudaError_t launch_extract_pose_features(const DecodeParams& params, const BoneQuery& query, const FeatureQuery& features, bool database,
 		cudaStream_t stream);
+	// feature_search.cu: the pack, one thread per output float; the search, which writes every result then atomicMin-s each block's best
+	cudaError_t configure_feature_search_kernels();
+	cudaError_t launch_pack_pose_features(const PackParams& params, cudaStream_t stream);
+	cudaError_t launch_search_pose_features(const SearchParams& params, int num_sms, cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

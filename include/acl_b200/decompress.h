@@ -549,6 +549,25 @@ namespace acl_b200
 				d_bone_lists, num_lists, bones_per_list, d_request_lists, d_root_tracks, d_parent_indices, d_skeleton_offsets, d_out, d_out_flags,
 				stream), "aclb200_extract_pose_features");
 		}
+		// Motion matching (aclb200_pack_pose_features): extract_pose_features rows of num_requests requests (S = num_offsets, K =
+		// bones_per_list) into vectors of num_dims floats, out[r][d] = (v_d - mean[d]) * scale[d] at d_out + r * out_stride floats. `terms`,
+		// `mean` and `scale` are host arrays (mean / scale nullptr: 0 / 1); pose_stride_bytes 0 = S * K rows.
+		void pack_pose_features(const void* d_rows, uint32_t num_requests, uint32_t num_offsets, uint32_t bones_per_list,
+			const aclb200_feature_term* terms, uint32_t num_terms, uint32_t num_dims, float* d_out, uint32_t out_stride, const float* mean = nullptr,
+			const float* scale = nullptr, uint64_t pose_stride_bytes = 0, void* stream = nullptr)
+		{
+			m_device->check(aclb200_pack_pose_features(m_device->get(), d_rows, num_requests, num_offsets, bones_per_list, pose_stride_bytes, terms,
+				num_terms, mean, scale, num_dims, d_out, out_stride, stream), "aclb200_pack_pose_features");
+		}
+		// Motion matching (aclb200_search_pose_features): the lowest cost allowed database row of each query (the lowest row on a tie,
+		// {ACLB200_NO_ROW, +inf} without one); strides in floats, d_row_tags nullptr: every row allowed by every tag mask.
+		void search_pose_features(const float* d_database, uint64_t num_rows, uint64_t db_stride, const float* d_query_vectors,
+			const aclb200_search_query* d_queries, uint32_t num_queries, uint64_t q_stride, uint32_t num_dims, aclb200_search_result* d_results,
+			const uint32_t* d_row_tags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_search_pose_features(m_device->get(), d_database, num_rows, db_stride, d_row_tags, d_query_vectors, d_queries,
+				num_queries, q_stride, num_dims, d_results, stream), "aclb200_search_pose_features");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 14
+#define ACLB200_VERSION_MINOR 15
 
 typedef enum aclb200_status
 {
@@ -782,6 +782,79 @@ ACLB200_API aclb200_status aclb200_extract_pose_features(aclb200_context* contex
 	const uint32_t* d_bone_lists, uint32_t num_lists, uint32_t bones_per_list, const uint32_t* d_request_lists,
 	const uint32_t* d_root_tracks, const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets,
 	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* ---- Motion matching: pose feature rows packed into vectors, and the best database row of each query ---------------------------- */
+
+/* aclb200_feature_term::kind */
+#define ACLB200_FEATURE_POSITION 0u		/* the translation of row (s0, k) */
+#define ACLB200_FEATURE_DIRECTION 1u	/* rtm::quat_mul_vector3(e_axis, rotation of row (s0, k)): where the bone's local axis points */
+#define ACLB200_FEATURE_VELOCITY 2u		/* (translation of row (s1, k) - translation of row (s0, k)) * inv_dt */
+/* The most dimensions of a packed feature vector */
+#define ACLB200_MAX_FEATURE_DIMS 64
+/* aclb200_search_result::row of a query without a candidate */
+#define ACLB200_NO_ROW 0xFFFFFFFFu
+
+/* One term of a feature vector: 1 to 3 of the x, y, z components of one vector taken from the rows of one request */
+typedef struct aclb200_feature_term
+{
+	uint32_t kind;				/* ACLB200_FEATURE_* */
+	uint32_t s0;				/* the offset of the row read (VELOCITY: the earlier one), 0..S-1 */
+	uint32_t s1;				/* VELOCITY: the offset of the later row, 0..S-1; unused otherwise */
+	uint32_t k;					/* the bone list entry, 0..K-1 */
+	uint32_t axis;				/* DIRECTION: 0, 1 or 2 = the unit x, y or z axis; unused otherwise */
+	uint32_t components;		/* bit mask of the components emitted, x = 1, y = 2, z = 4 (1..7), always in x, y, z order */
+	float    inv_dt;			/* VELOCITY: 1 / the time between the two offsets; unused otherwise */
+} aclb200_feature_term;
+
+/* Pack pose features into vectors: request r's rows of aclb200_extract_pose_features (S = num_offsets, K = bones_per_list; row (s, k) at
+ * d_rows + r * pose_stride + (s * K + k) * 48, pose_stride = pose_stride_bytes, 0 = S * K * 48, 16 byte aligned) become one vector of D =
+ * num_dims floats at d_out + r * out_stride. The terms (a HOST array of num_terms, copied into the launch) emit their components in array
+ * order, each term its components in x, y, z order; D must be the sum of their component counts.
+ *   POSITION    v = t(s0, k)_c
+ *   DIRECTION   v = rtm::quat_mul_vector3(e_axis, q(s0, k))_c, the rotation function of the object space walk
+ *   VELOCITY    v = (t(s1, k)_c - t(s0, k)_c) * inv_dt, an IEEE subtract then multiply, not fused
+ *   out[r][d]   (v_d - mean[d]) * scale[d], not fused; mean and scale are HOST float[D], NULL reads as 0 and 1 with the same arithmetic.
+ * out_stride is in floats, at least D and a multiple of 4; d_out is 16 byte aligned; the floats from D to out_stride are not written. The
+ * pack does not know which rows extract_pose_features left untouched: a caller tags such requests' database rows out of the search.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: an unknown kind, s0 or s1 >= S, k >= K, axis > 2, components 0 or above 7,
+ * a non-finite inv_dt, mean or scale, num_terms 0 or NULL terms, D not the sum of the terms' components or above ACLB200_MAX_FEATURE_DIMS,
+ * num_offsets 0 or above ACLB200_MAX_FEATURE_OFFSETS, bones_per_list 0 or above ACLB200_MAX_QUERY_BONES, a pose stride below S * K * 48 or
+ * not a multiple of 16, NULL or misaligned d_rows or d_out with num_requests > 0. */
+ACLB200_API aclb200_status aclb200_pack_pose_features(aclb200_context* context, const void* d_rows, uint32_t num_requests, uint32_t num_offsets,
+	uint32_t bones_per_list, uint64_t pose_stride_bytes, const aclb200_feature_term* terms, uint32_t num_terms, const float* mean,
+	const float* scale, uint32_t num_dims, float* d_out, uint32_t out_stride, void* stream);
+
+/* What one query searches */
+typedef struct aclb200_search_query
+{
+	uint32_t tag_mask;			/* row r is allowed when (d_row_tags[r] & tag_mask) != 0 */
+	uint32_t exclude_begin;		/* rows exclude_begin <= r < exclude_end are skipped (the clip and time the character plays now); */
+	uint32_t exclude_end;		/* begin >= end skips nothing */
+} aclb200_search_query;
+
+/* A query's best row. Read as a little endian uint64 it is (cost bits << 32) | row, the key the search minimises. */
+typedef struct aclb200_search_result
+{
+	uint32_t row;				/* ACLB200_NO_ROW when the query has no candidate */
+	float    cost;				/* +inf when the query has no candidate */
+} aclb200_search_result;
+
+/* The best database row of each query, exact and tie-stable, in one pass over the database. Database row r is D = num_dims floats at
+ * d_database + r * db_stride (r < num_rows), query q's vector at d_query_vectors + q * q_stride.
+ *   cost        acc = +0.0f; for d = 0 .. D-1 in order: diff = q[d] - x[d] (IEEE subtract); acc = fmaf(diff, diff, acc), a fused multiply add
+ *               (correctly rounded, as C's fmaf). Never negative.
+ *   candidate   row r with exclude_begin <= r < exclude_end false, (tag[r] & tag_mask) != 0 and a cost that is not NaN (+inf is a candidate);
+ *               tag[r] = d_row_tags[r] (device uint32[num_rows]), every tag 0xFFFFFFFF when d_row_tags is NULL.
+ *   result      d_results[q] (device, 8 byte aligned) = the candidate with the smallest cost, the lowest row among equal costs; {ACLB200_NO_ROW,
+ *               +inf} without a candidate (every query when num_rows is 0).
+ * The result does not depend on the launch shape or the order blocks run in: two launches give the same bits. d_queries is device
+ * aclb200_search_query[num_queries].
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing and leaving d_results untouched: D 0 or above ACLB200_MAX_FEATURE_DIMS, a
+ * stride below D or not a multiple of 4 floats, vectors not 16 byte aligned, results not 8 byte aligned, num_rows >= 2^32 - 1, NULL
+ * d_database with num_rows > 0, NULL d_query_vectors, d_queries or d_results with num_queries > 0. */
+ACLB200_API aclb200_status aclb200_search_pose_features(aclb200_context* context, const float* d_database, uint64_t num_rows, uint64_t db_stride,
+	const uint32_t* d_row_tags, const float* d_query_vectors, const aclb200_search_query* d_queries, uint32_t num_queries, uint64_t q_stride,
+	uint32_t num_dims, aclb200_search_result* d_results, void* stream);
 
 /* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
  * aclb200_apply_additive_to_base): num_poses poses of rtm::qvvf rows of one skeleton (48 byte bones, 16 byte aligned, pose p at
