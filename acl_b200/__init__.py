@@ -23,4 +23,5 @@ from .api import (  # noqa: F401
     FEATURE_CLAMP, FEATURE_LOOP, MAX_FEATURE_OFFSETS, FEATURE_REQUEST_DTYPE, make_feature_requests,
     FEATURE_POSITION, FEATURE_DIRECTION, FEATURE_VELOCITY, MAX_FEATURE_DIMS, NO_ROW, FEATURE_TERM_DTYPE, SEARCH_QUERY_DTYPE,
     SEARCH_RESULT_DTYPE, make_feature_terms, feature_term_dims, make_search_queries,
+    NO_INERTIALIZATION, INERTIALIZATION_DTYPE, make_inertializations, INERTIALIZED_REQUEST_DTYPE, make_inertialized_requests,
 )

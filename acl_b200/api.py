@@ -178,6 +178,10 @@ def _lib():
         l.aclb200_extract_pose_features.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp]
         l.aclb200_pack_pose_features.argtypes = [vp, vp, u32, u32, u32, u64, vp, u32, vp, vp, u32, vp, u32, vp]
         l.aclb200_search_pose_features.argtypes = [vp, vp, u64, u64, vp, vp, vp, u32, u64, u32, vp, vp]
+        l.aclb200_begin_inertialization.argtypes = [vp, vp, vp, vp, vp, u64, u32, u64, C.c_float, vp, u64, vp, vp]
+        l.aclb200_inertialize_poses.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, u64, u64, vp]
+        l.aclb200_decompress_tracks_inertialized.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u64, u64, vp, vp, u32, vp, vp, vp]
+        l.aclb200_decompress_tracks_inertialized_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u64, u64, vp, vp, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -210,6 +214,8 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_layered", "aclb200_decompress_tracks_layered_skinning",
         "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
         "aclb200_extract_root_motion", "aclb200_extract_pose_features", "aclb200_pack_pose_features", "aclb200_search_pose_features",
+        "aclb200_begin_inertialization", "aclb200_inertialize_poses", "aclb200_decompress_tracks_inertialized",
+        "aclb200_decompress_tracks_inertialized_skinning",
     ]
 
 
@@ -272,6 +278,10 @@ FEATURE_TERM_DTYPE = np.dtype([("kind", np.uint32), ("s0", np.uint32), ("s1", np
                                ("components", np.uint32), ("inv_dt", np.float32)])
 SEARCH_QUERY_DTYPE = np.dtype([("tag_mask", np.uint32), ("exclude_begin", np.uint32), ("exclude_end", np.uint32)])
 SEARCH_RESULT_DTYPE = np.dtype([("row", np.uint32), ("cost", np.float32)])
+NO_INERTIALIZATION = 0xFFFFFFFF  # an inertialization that reads no record
+INERTIALIZATION_DTYPE = np.dtype([("record", np.uint32), ("elapsed", np.float32), ("halflife", np.float32)])
+INERTIALIZED_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("record", np.uint32), ("elapsed", np.float32),
+                                       ("halflife", np.float32)])
 
 
 def make_layers(clips, times, ops, weights) -> np.ndarray:
@@ -327,6 +337,27 @@ def make_feature_terms(kinds, s0, k, components=7, s1=0, axis=0, inv_dt=0.0) -> 
 def feature_term_dims(terms: np.ndarray) -> int:
     """D of a term array: the number of components its masks emit"""
     return int(sum(bin(int(c) & 7).count("1") for c in np.asarray(terms)["components"]))
+
+
+def make_inertializations(records, elapsed, halflife) -> np.ndarray:
+    """(record index or NO_INERTIALIZATION, seconds since the capture, halflife in seconds) arrays, or anything that broadcasts to one
+    shape -> aclb200_inertialization[]"""
+    records, elapsed, halflife = np.broadcast_arrays(np.asarray(records, dtype=np.uint32), np.asarray(elapsed, dtype=np.float32),
+                                                     np.asarray(halflife, dtype=np.float32))
+    out = np.empty(records.shape, dtype=INERTIALIZATION_DTYPE)
+    out["record"], out["elapsed"], out["halflife"] = records, elapsed, halflife
+    return out.reshape(-1)
+
+
+def make_inertialized_requests(clips, times, records, elapsed, halflife) -> np.ndarray:
+    """(clip index, sample time, record index or NO_INERTIALIZATION, seconds since the capture, halflife in seconds) arrays, or anything
+    that broadcasts to one shape -> aclb200_inertialized_request[]"""
+    fields = np.broadcast_arrays(np.asarray(clips, dtype=np.uint32), np.asarray(times, dtype=np.float32), np.asarray(records, dtype=np.uint32),
+                                 np.asarray(elapsed, dtype=np.float32), np.asarray(halflife, dtype=np.float32))
+    out = np.empty(fields[0].shape, dtype=INERTIALIZED_REQUEST_DTYPE)
+    for name, value in zip(INERTIALIZED_REQUEST_DTYPE.names, fields):
+        out[name] = value
+    return out.reshape(-1)
 
 
 def make_search_queries(tag_masks=0xFFFFFFFF, exclude_begin=0, exclude_end=0) -> np.ndarray:
@@ -779,6 +810,46 @@ class Context:
         either input."""
         self._check(_lib().aclb200_blend_poses(self._handle, _device_ptr(d_from_poses), _device_ptr(d_to_poses), _device_ptr(d_out), num_poses,
                                                num_tracks, pose_stride_bytes, weight, _device_ptr(d_weights), _stream_ptr(stream)))
+
+    def begin_inertialization(self, d_src, d_src_prev, d_dst, d_dst_prev, num_transitions: int, num_tracks: int, inv_dt: float, d_records,
+                              d_record_slots=None, pose_stride_bytes: int = 0, record_stride_bytes: int = 0, stream=None) -> None:
+        """The inertialization record of each transition: from the displayed QVV48 poses this frame and the frame before (d_src,
+        d_src_prev) and the destination poses (d_dst, d_dst_prev), one frame being 1 / inv_dt seconds. Transition j writes the record at
+        slot d_record_slots[j] (uint32), or j, of d_records (float32, num_tracks * 16 floats per record unless record_stride_bytes)."""
+        self._check(_lib().aclb200_begin_inertialization(self._handle, _device_ptr(d_src), _device_ptr(d_src_prev), _device_ptr(d_dst),
+                                                         _device_ptr(d_dst_prev), num_transitions, num_tracks, pose_stride_bytes, inv_dt,
+                                                         _device_ptr(d_records), record_stride_bytes, _device_ptr(d_record_slots),
+                                                         _stream_ptr(stream)))
+
+    def inertialize_poses(self, d_poses, d_out, num_poses: int, num_tracks: int, d_inertializations, d_records, num_records: int,
+                          pose_stride_bytes: int = 0, record_stride_bytes: int = 0, stream=None) -> None:
+        """Each QVV48 pose with its record's offset decayed onto it (d_inertializations: INERTIALIZATION_DTYPE bytes, one per pose). A
+        pose whose record is NO_INERTIALIZATION is copied unchanged, one whose record is >= num_records is not written; d_out may be
+        d_poses."""
+        self._check(_lib().aclb200_inertialize_poses(self._handle, _device_ptr(d_poses), _device_ptr(d_out), num_poses, num_tracks,
+                                                     pose_stride_bytes, _device_ptr(d_inertializations), _device_ptr(d_records), num_records,
+                                                     record_stride_bytes, _stream_ptr(stream)))
+
+    def decompress_tracks_inertialized(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, d_records,
+                                       num_records: int, record_stride_bytes: int = 0, d_parent_indices=None, kind: int = 0,
+                                       d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """num_requests inertialized requests (make_inertialized_requests): each pose decoded, then its record's offset decayed onto it in
+        the same launch (NO_INERTIALIZATION: the plain decode's rows; a record >= num_records: nothing written). With d_parent_indices the
+        pose leaves in object space as `kind` rows (OBJECT_*); without, in options.output_layout."""
+        self._check(_lib().aclb200_decompress_tracks_inertialized(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                  C.byref(options), _device_ptr(d_records), num_records, record_stride_bytes,
+                                                                  _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets), kind,
+                                                                  _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def decompress_tracks_inertialized_skinning(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices,
+                                                d_inverse_bind, d_out, d_records, num_records: int, record_stride_bytes: int = 0,
+                                                d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """decompress_tracks_inertialized's poses as skinning rows, with the clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_inertialized_skinning(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                           C.byref(options), _device_ptr(d_records), num_records,
+                                                                           record_stride_bytes, _device_ptr(d_parent_indices),
+                                                                           _device_ptr(d_skeleton_offsets), _device_ptr(d_inverse_bind),
+                                                                           _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
 
     # ---- host buffers in, host buffers out (the call the C++ header shim uses) ----
     def decompress_tracks_host(self, clipset: ClipSet, requests: np.ndarray, options: Options, out: np.ndarray) -> np.ndarray:

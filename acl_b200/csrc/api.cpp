@@ -42,6 +42,10 @@ namespace aclb200
 			const float* d_bone_masks;				// [num_masks][mask_stride]
 			uint32_t num_masks;
 			uint32_t mask_stride;					// resolved by check_layer_masks (0 = max_tracks)
+			// inertialize: the records (every field 0 in the other modes)
+			const void* d_records;
+			uint64_t record_stride;					// resolved by check_records (0 = max_tracks * 64)
+			uint64_t num_records;
 		};
 		const char* const k_pose_unfit = ": one pose does not fit in a block's shared memory";
 		const char* const k_pair_unfit = ": the two poses of a pair do not fit in a block's shared memory";
@@ -228,6 +232,17 @@ namespace aclb200
 		return ACLB200_OK;
 	}
 
+	// inertialization records: 64 byte entries per bone, 16 byte aligned; record_stride 0 becomes num_tracks * 64
+	aclb200_status check_records(aclb200_context* context, const void* d_records, uint32_t num_tracks, uint64_t& record_stride, const char* what)
+	{
+		if (record_stride == 0)
+			record_stride = uint64_t(num_tracks) * ACLB200_INERTIALIZATION_ENTRY_BYTES;
+		if (record_stride < uint64_t(num_tracks) * ACLB200_INERTIALIZATION_ENTRY_BYTES || (record_stride % 16) != 0
+			|| (reinterpret_cast<uintptr_t>(d_records) % 16) != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": records are 64 byte entries per bone, 16 byte aligned");
+		return ACLB200_OK;
+	}
+
 	aclb200_status check_inverse_binds(aclb200_context* context, const float* d_inverse_bind, const char* what)
 	{
 		if (d_inverse_bind == nullptr || (reinterpret_cast<uintptr_t>(d_inverse_bind) % 16) != 0)
@@ -320,6 +335,9 @@ namespace aclb200
 			params.bone_masks = composed.d_bone_masks;
 			params.num_masks = composed.num_masks;
 			params.mask_stride = composed.mask_stride;
+			params.records = static_cast<const uint8_t*>(composed.d_records);
+			params.record_stride = composed.record_stride;
+			params.num_records = uint32_t(composed.num_records);
 			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 			return launch_clearing_flags(context, d_out_flags, cuda_stream, entry.c_str(), entry.c_str(),
 				[&] { return launch_transform_decompress_tracks(params, composed.compose, params.db_tiers != nullptr, cuda_stream); });
@@ -392,6 +410,33 @@ namespace aclb200
 			return decompress_composed(context, clipset, d_layers, num_poses, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
 				skinning, d_inverse_bind, d_out, d_out_flags, stream);
 		}
+
+		// the inertialized decode and its _skinning sibling: the record checks, then the composed path (requests are 20 byte records)
+		aclb200_status decompress_inertialized(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_inertialized_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_inertialized_skinning" : "decompress_tracks_inertialized";
+			if (context == nullptr || clipset == nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
+			if (num_records >= uint64_t(ACLB200_NO_INERTIALIZATION))
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": num_records must be below 2^32 - 1");
+			if (num_records != 0 && d_records == nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": null record pointer");
+			static_assert(sizeof(aclb200_inertialized_request) == 20 && offsetof(aclb200_inertialized_request, inertialization) == 8,
+				"an inertialized request is a request and its inertialization, five words");
+			Composed composed = { what, k_pose_unfit, k_compose_inertialize, 1 };
+			composed.record_stride = record_stride_bytes;
+			const aclb200_status status = check_records(context, num_records != 0 ? d_records : nullptr, clipset->info.max_tracks,
+				composed.record_stride, what);
+			if (status != ACLB200_OK)
+				return status;
+			composed.d_records = d_records;
+			composed.num_records = num_records;
+			return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
+		}
 	}
 }
 
@@ -401,7 +446,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.15 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.16 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -1000,6 +1045,102 @@ extern "C"
 		return finish_launch(context, launch_blend_poses(static_cast<const uint8_t*>(d_from_poses), static_cast<const uint8_t*>(d_to_poses),
 			static_cast<uint8_t*>(d_out), num_poses, num_tracks, stride, weight, d_weights, context->num_sms, static_cast<cudaStream_t>(stream)),
 			"blend_poses");
+	}
+
+	aclb200_status aclb200_begin_inertialization(aclb200_context* context, const void* d_src, const void* d_src_prev, const void* d_dst,
+		const void* d_dst_prev, uint64_t num_transitions, uint32_t num_tracks, uint64_t pose_stride_bytes, float inv_dt, void* d_records,
+		uint64_t record_stride_bytes, const uint32_t* d_record_slots, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		if (!std::isfinite(inv_dt) || inv_dt == 0.0f)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "begin_inertialization: inv_dt must be finite and not zero");
+		if (num_transitions == 0 || num_tracks == 0)
+			return ACLB200_OK;
+		if (d_src == nullptr || d_src_prev == nullptr || d_dst == nullptr || d_dst_prev == nullptr || d_records == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "begin_inertialization: null pose or record pointer");
+		uint64_t stride = pose_stride_bytes;
+		aclb200_status status = check_qvvf_rows(context, { d_src, d_src_prev, d_dst, d_dst_prev }, num_tracks, stride, "begin_inertialization");
+		if (status != ACLB200_OK)
+			return status;
+		uint64_t record_stride = record_stride_bytes;
+		status = check_records(context, d_records, num_tracks, record_stride, "begin_inertialization");
+		if (status != ACLB200_OK)
+			return status;
+		if (reinterpret_cast<uintptr_t>(d_record_slots) % 4 != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "begin_inertialization: record slots must be 4 byte aligned");
+		InertializationCapture capture = {};
+		capture.src = static_cast<const uint8_t*>(d_src);
+		capture.src_prev = static_cast<const uint8_t*>(d_src_prev);
+		capture.dst = static_cast<const uint8_t*>(d_dst);
+		capture.dst_prev = static_cast<const uint8_t*>(d_dst_prev);
+		capture.records = static_cast<uint8_t*>(d_records);
+		capture.record_slots = d_record_slots;
+		capture.num_transitions = num_transitions;
+		capture.pose_stride = stride;
+		capture.record_stride = record_stride;
+		capture.num_tracks = num_tracks;
+		capture.inv_dt = inv_dt;
+		cudaSetDevice(context->device);
+		return finish_launch(context, launch_begin_inertialization(capture, context->num_sms, static_cast<cudaStream_t>(stream)), "begin_inertialization");
+	}
+
+	aclb200_status aclb200_inertialize_poses(aclb200_context* context, const void* d_poses, void* d_out, uint64_t num_poses,
+		uint32_t num_tracks, uint64_t pose_stride_bytes, const aclb200_inertialization* d_inertializations, const void* d_records,
+		uint64_t num_records, uint64_t record_stride_bytes, void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		if (num_records >= uint64_t(ACLB200_NO_INERTIALIZATION))
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "inertialize_poses: num_records must be below 2^32 - 1");
+		uint64_t record_stride = record_stride_bytes;
+		aclb200_status status = check_records(context, num_records != 0 ? d_records : nullptr, num_tracks, record_stride, "inertialize_poses");
+		if (status != ACLB200_OK)
+			return status;
+		if (num_poses == 0 || num_tracks == 0)
+			return ACLB200_OK;
+		if (d_poses == nullptr || d_out == nullptr || d_inertializations == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "inertialize_poses: null pose or inertialization pointer");
+		if (reinterpret_cast<uintptr_t>(d_inertializations) % 4 != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "inertialize_poses: inertializations must be 4 byte aligned");
+		if (num_records != 0 && d_records == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "inertialize_poses: null record pointer");
+		uint64_t stride = pose_stride_bytes;
+		status = check_qvvf_rows(context, { d_poses, d_out }, num_tracks, stride, "inertialize_poses");
+		if (status != ACLB200_OK)
+			return status;
+		InertializationApply apply = {};
+		apply.poses = static_cast<const uint8_t*>(d_poses);
+		apply.out = static_cast<uint8_t*>(d_out);
+		apply.inertializations = d_inertializations;
+		apply.records = static_cast<const uint8_t*>(d_records);
+		apply.num_poses = num_poses;
+		apply.pose_stride = stride;
+		apply.record_stride = record_stride;
+		apply.num_records = num_records;
+		apply.num_tracks = num_tracks;
+		cudaSetDevice(context->device);
+		return finish_launch(context, launch_inertialize_poses(apply, context->num_sms, static_cast<cudaStream_t>(stream)), "inertialize_poses");
+	}
+
+	aclb200_status aclb200_decompress_tracks_inertialized(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		return decompress_inertialized(context, clipset, d_requests, num_requests, options, d_records, num_records, record_stride_bytes,
+			d_parent_indices, d_skeleton_offsets, object_kind, false, nullptr, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_tracks_inertialized_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		return decompress_inertialized(context, clipset, d_requests, num_requests, options, d_records, num_records, record_stride_bytes,
+			d_parent_indices, d_skeleton_offsets, ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_local_to_skinning(aclb200_context* context, const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks,

@@ -196,6 +196,11 @@ namespace aclb200
 		const float* bone_masks;					// [num_masks][mask_stride] one weight per bone of the base clip
 		uint32_t num_masks;							// at most k_max_layer_masks
 		uint32_t mask_stride;
+		// the inertialized decode (aclb200_decompress_tracks_inertialized, k_compose_inertialize): `requests` holds 20 byte
+		// aclb200_inertialized_request records
+		const uint8_t* records;						// record r at records + r * record_stride, 64 bytes per bone
+		uint64_t record_stride;
+		uint32_t num_records;						// < 2^32 - 1
 	};
 
 	// The bone query (aclb200_decompress_bones, bones.cu): the lists, the skeletons and the launch's shared memory carve-up. A kernel
@@ -278,13 +283,46 @@ namespace aclb200
 		uint32_t num_dims;
 	};
 
+	// The inertialization capture (aclb200_begin_inertialization, inertialization.cu): transition j's four QVV48 poses at j * pose_stride,
+	// its record at records + (record_slots ? record_slots[j] : j) * record_stride, 64 bytes per bone
+	struct InertializationCapture
+	{
+		const uint8_t* src;
+		const uint8_t* src_prev;
+		const uint8_t* dst;
+		const uint8_t* dst_prev;
+		uint8_t* records;
+		const uint32_t* record_slots;
+		uint64_t num_transitions;
+		uint64_t pose_stride;
+		uint64_t record_stride;
+		uint32_t num_tracks;
+		float inv_dt;
+	};
+
+	// The inertialization apply (aclb200_inertialize_poses, inertialization.cu): pose p at p * pose_stride in poses and out, decayed with
+	// inertializations[p]
+	struct InertializationApply
+	{
+		const uint8_t* poses;
+		uint8_t* out;
+		const aclb200_inertialization* inertializations;
+		const uint8_t* records;
+		uint64_t num_poses;
+		uint64_t pose_stride;
+		uint64_t record_stride;
+		uint64_t num_records;					// < 2^32 - 1
+		uint32_t num_tracks;
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
 	// (aclb200_decompress_tracks_layered). layers_masked: the layers mode with bone masks and weighted ADDITIVE layers
-	// (aclb200_decompress_tracks_layered_masked).
+	// (aclb200_decompress_tracks_layered_masked). inertialize: each request's pose with its inertialization record's offset decayed onto
+	// it (aclb200_decompress_tracks_inertialized).
 	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_layers = 4,
-		k_compose_layers_masked = 5, k_compose_count = 6 };
+		k_compose_layers_masked = 5, k_compose_inertialize = 6, k_compose_count = 7 };
 
 	// the deepest layer stack of aclb200_decompress_tracks_layered
 	constexpr uint32_t k_max_layers = 8;
@@ -310,6 +348,8 @@ namespace aclb200
 		uint64_t pose_stride, uint32_t additive_format, uint32_t* flags, int num_sms, cudaStream_t stream);
 	cudaError_t launch_blend_poses(const uint8_t* from_poses, const uint8_t* to_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks,
 		uint64_t pose_stride, float weight, const float* weights, int num_sms, cudaStream_t stream);
+	// the grid of the pose operations: one thread per (pose, bone), at most 16 blocks of 256 threads per SM, which loop over the rest
+	uint32_t pose_operation_blocks(uint64_t num_poses, uint32_t num_tracks, int num_sms);
 	// aclb200_local_to_skinning: one warp per pose, the pose staged in shared memory; 0 warps per block when one pose does not fit
 	uint32_t local_to_skinning_warps(uint32_t num_tracks, int max_dynamic_smem);
 	cudaError_t launch_local_to_skinning(const uint8_t* local_poses, uint8_t* out, uint64_t num_poses, uint32_t num_tracks, uint64_t pose_stride,
@@ -335,6 +375,9 @@ namespace aclb200
 	cudaError_t configure_feature_search_kernels();
 	cudaError_t launch_pack_pose_features(const PackParams& params, cudaStream_t stream);
 	cudaError_t launch_search_pose_features(const SearchParams& params, int num_sms, cudaStream_t stream);
+	// inertialization.cu: the capture and the apply, one thread per (pose, bone)
+	cudaError_t launch_begin_inertialization(const InertializationCapture& capture, int num_sms, cudaStream_t stream);
+	cudaError_t launch_inertialize_poses(const InertializationApply& apply, int num_sms, cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

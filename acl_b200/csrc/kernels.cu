@@ -49,6 +49,16 @@ namespace aclb200
 			uint32_t num_stacks;
 		};
 		static_assert(sizeof(LayerSlot) == 16, "a layer slot is 16 bytes beside each request state");
+
+		// The inertialized decode keeps each request's aclb200_inertialization in the same 16 byte slot beside its state
+		struct alignas(16) InertializationSlot
+		{
+			uint32_t record;
+			float    elapsed;
+			float    halflife;
+			uint32_t unused;
+		};
+		static_assert(sizeof(InertializationSlot) == sizeof(LayerSlot), "an inertialization slot takes a layer slot's place");
 		constexpr uint32_t k_layer_base = 3, k_layer_unknown = 4, k_no_base = 0xFFFFFFFFu;
 		constexpr uint32_t k_layer_op_mask = (1u << k_layer_op_bits) - 1;
 
@@ -84,6 +94,10 @@ namespace aclb200
 		//             k_compose_layers_masked (aclb200_decompress_tracks_layered_masked): the layered mode where each layer may carry a bone
 		//             mask (its weight times mask[bone], skipped where the mask is +-0) and ADDITIVE layers take their weight. A mode of its
 		//             own rather than a run-time switch of k_compose_layers: the switch made the unmasked fold 1.4 % slower on C2.
+		//             k_compose_inertialize (aclb200_decompress_tracks_inertialized): requests are 20 byte aclb200_inertialized_request
+		//             records; a request whose record is at or above p.num_records is not sought (it writes nothing). Phase 4c decays the
+		//             record's offset onto each bone's row in place (obj::inertialize_row); ACLB200_NO_INERTIALIZATION rows are left as
+		//             decoded. Phases 4b and 5 then run as for the object mode when parents are given, and store local rows without them.
 		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
@@ -91,6 +105,7 @@ namespace aclb200
 			constexpr bool PAIRED = COMPOSE == k_compose_additive || COMPOSE == k_compose_blend;
 			constexpr bool MASKED = COMPOSE == k_compose_layers_masked;
 			constexpr bool LAYERED = COMPOSE == k_compose_layers || MASKED;
+			constexpr bool INERT = COMPOSE == k_compose_inertialize;
 			// MASKED: a layer slot's op carries the layer's mask index above its low k_layer_op_bits
 			auto slot_op = [](uint32_t slot) { return MASKED ? slot & k_layer_op_mask : slot; };
 			static_assert(COMPOSE == k_compose_local || OUT_STAGED, "the composed decodes work on poses assembled in shared memory");
@@ -112,6 +127,7 @@ namespace aclb200
 			auto first_stack = [&]() { return blockIdx.x * fast_div(p.requests_per_block, p.magic_layers); };
 			if (LAYERED && threadIdx.x == 0)
 				s_layer[0].num_stacks = fast_div(num_requests, p.magic_layers);
+			InertializationSlot* s_inert = reinterpret_cast<InertializationSlot*>(s_layer);
 
 			if (STAGED)
 			{
@@ -146,6 +162,16 @@ namespace aclb200
 					rs.num_tracks = 0;
 					if (layer.op == ACLB200_LAYER_BLEND || layer.op == ACLB200_LAYER_ADDITIVE)
 						seek_request<DB>(p, layer.pose, first_stack() + stack, rs);
+				}
+				else if constexpr (INERT)
+				{
+					// {clip, sample_time, record, elapsed, halflife}, five words at 4 byte alignment
+					const uint32_t* words = reinterpret_cast<const uint32_t*>(p.requests) + uint64_t(first_request + threadIdx.x) * 5;
+					const uint32_t record = __ldg(words + 2);
+					rs.num_tracks = 0;
+					if (record == ACLB200_NO_INERTIALIZATION || record < p.num_records)
+						seek_request<DB>(p, aclb200_request{ __ldg(words), __uint_as_float(__ldg(words + 1)) }, first_request + threadIdx.x, rs);
+					s_inert[threadIdx.x] = InertializationSlot{ record, __uint_as_float(__ldg(words + 3)), __uint_as_float(__ldg(words + 4)), 0u };
 				}
 				else
 					seek_transform<DB, RS, PAIRED>(p, first_request + threadIdx.x, rs);
@@ -369,11 +395,31 @@ namespace aclb200
 				}
 			}
 
+			// ---- phase 4c, inertialize: one thread per (request, bone) decays the request's record entry onto the row, in place ----
+			if constexpr (INERT)
+			{
+				__syncthreads();
+				const uint32_t num_slots = num_requests * p.max_tracks;
+				for (uint32_t slot = threadIdx.x; slot < num_slots; slot += k_threads_per_block)
+				{
+					const uint32_t local_request = fast_div(slot, p.magic_tracks);
+					const uint32_t bone = slot - local_request * p.max_tracks;
+					const InertializationSlot inertialization = s_inert[local_request];
+					if (bone >= s_req[local_request].num_tracks || inertialization.record == ACLB200_NO_INERTIALIZATION)
+						continue;
+					uint8_t* row = s_out + size_t(local_request) * p.smem_pose_bytes + size_t(bone) * p.bone_stride;
+					const float4* entry = reinterpret_cast<const float4*>(p.records + uint64_t(inertialization.record) * p.record_stride
+						+ uint64_t(bone) * ACLB200_INERTIALIZATION_ENTRY_BYTES);
+					obj::inertialize_row(row, row, entry, obj::inertialization_decay(inertialization.elapsed, inertialization.halflife),
+						p.layout == ACLB200_LAYOUT_QVV40);
+				}
+			}
+
 			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (PAIRED: the
 			// combined row of each pair, when parents are given) ----
 			if constexpr (COMPOSE != k_compose_local)
 			{
-				if ((!PAIRED && !LAYERED) || p.parent_indices != nullptr)
+				if ((!PAIRED && !LAYERED && !INERT) || p.parent_indices != nullptr)
 				{
 					__syncthreads();
 					uint32_t flags = 0;
@@ -1036,13 +1082,12 @@ namespace aclb200
 			if (lane == 0 && flags != 0 && out_flags != nullptr)
 				atomicOr(out_flags, flags);
 		}
+	}
 
-		// the pose operations: one thread per (pose, bone), at most 16 blocks of 256 threads per SM, which loop over the rest
-		uint32_t pose_operation_blocks(uint64_t num_poses, uint32_t num_tracks, int num_sms)
-		{
-			const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
-			return uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
-		}
+	uint32_t pose_operation_blocks(uint64_t num_poses, uint32_t num_tracks, int num_sms)
+	{
+		const uint64_t blocks_needed = (num_poses * num_tracks + 255) / 256;
+		return uint32_t(blocks_needed < uint64_t(num_sms) * 16 ? blocks_needed : uint64_t(num_sms) * 16);
 	}
 
 	// Called once per context: lets the staged kernels use large dynamic shared memory windows. `max_dynamic_smem` comes in as the
@@ -1087,7 +1132,8 @@ namespace aclb200
 		const bool force_output_staging = compose != k_compose_local;
 		const bool pairs = compose == k_compose_additive || compose == k_compose_blend;
 		const bool layers = compose == k_compose_layers || compose == k_compose_layers_masked;
-		const uint32_t state_bytes = (database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState))) + (layers ? uint32_t(sizeof(LayerSlot)) : 0u);
+		const bool slots = layers || compose == k_compose_inertialize;		// a LayerSlot or an InertializationSlot beside each request state
+		const uint32_t state_bytes = (database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState))) + (slots ? uint32_t(sizeof(LayerSlot)) : 0u);
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);
 		// ~28 KB of shared memory per block keeps 8 blocks resident per SM

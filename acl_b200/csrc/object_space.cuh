@@ -707,6 +707,184 @@ namespace aclb200
 					lerp_lane(fp, from.scale.z, to.scale.z, weight) };
 				store_pose_row(out_row, out, qvv40);
 			}
+
+			// ---- inertialization (aclb200_begin_inertialization, aclb200_inertialize_poses): rtm's quat_rotation_log and quat_rotation_exp
+			// (quatf.h:1306-1375) on their SSE2 paths, which are polynomials and IEEE operations only, so they match the reference on any CPU.
+			// rtm's float constants are static_cast<float> of its double literals (constants.h:35-47) ----
+			constexpr float k_rtm_pi = float(3.141592653589793238462643383279502884);
+			constexpr float k_rtm_half_pi = float(1.570796326794896619231321691639751442);
+			constexpr float k_rtm_two_pi = float(6.283185307179586476925286766559005768);
+			constexpr float k_rtm_one_div_two_pi = float(1.591549430918953357688837633725143620e-01);
+
+			// rtm::scalar_acos, scalarf.h:1142-1174: a degree 7 polynomial in |v| times sqrt(1 - |v|), reflected for v < 0
+			__device__ __forceinline__ float rtm_acos(float v)
+			{
+				const Fp<float> fp{};
+				const float x = fabsf(v);
+				float r = fp.add(fp.mul(x, -1.2690614339589956e-3f), 6.7072304676685235e-3f);
+				r = fp.sub(fp.mul(r, x), 1.7162031184398074e-2f);
+				r = fp.add(fp.mul(r, x), 3.0961594977611639e-2f);
+				r = fp.sub(fp.mul(r, x), 5.0207843052845647e-2f);
+				r = fp.add(fp.mul(r, x), 8.8986946573346160e-2f);
+				r = fp.sub(fp.mul(r, x), 2.1459960076929829e-1f);
+				r = fp.add(fp.mul(r, x), 1.5707963267948966f);
+				r = fp.mul(r, __fsqrt_rn(fp.sub(1.0f, x)));
+				return v < 0.0f ? fp.sub(k_rtm_pi, r) : r;
+			}
+
+			// the range reduction of rtm::scalar_sin and scalar_cos (scalarf.h:855-967): angle - bankers_round(angle / 2 pi) * 2 pi (roundss
+			// under SSE4.1, rint here), then reflected about copysign(pi, x) when |x| > pi / 2 (the compare is false for NaN)
+			__device__ __forceinline__ float rtm_reduce_angle(float angle, bool& within_half_pi)
+			{
+				const Fp<float> fp{};
+				const float x = fp.sub(angle, fp.mul(rintf(fp.mul(angle, k_rtm_one_div_two_pi)), k_rtm_two_pi));
+				within_half_pi = fabsf(x) <= k_rtm_half_pi;
+				return within_half_pi ? x : fp.sub(copysignf(k_rtm_pi, x), x);
+			}
+
+			// rtm::scalar_sin (SSE2 path): a degree 11 polynomial
+			__device__ __forceinline__ float rtm_sin(float angle)
+			{
+				const Fp<float> fp{};
+				bool within_half_pi;
+				const float x = rtm_reduce_angle(angle, within_half_pi);
+				const float x2 = fp.mul(x, x);
+				float r = fp.add(fp.mul(x2, -2.3828544692960918e-8f), 2.7521557770526783e-6f);
+				r = fp.sub(fp.mul(r, x2), 1.9840782426250314e-4f);
+				r = fp.add(fp.mul(r, x2), 8.3333303183525942e-3f);
+				r = fp.sub(fp.mul(r, x2), 1.6666666601721269e-1f);
+				r = fp.add(fp.mul(r, x2), 1.0f);
+				return fp.mul(r, x);
+			}
+
+			// rtm::scalar_cos (SSE2 path): a degree 10 polynomial whose sign bit is set (OR-ed, not flipped) when the angle was reflected
+			__device__ __forceinline__ float rtm_cos(float angle)
+			{
+				const Fp<float> fp{};
+				bool within_half_pi;
+				const float x = rtm_reduce_angle(angle, within_half_pi);
+				const float x2 = fp.mul(x, x);
+				float r = fp.add(fp.mul(x2, -2.6051615464872668e-7f), 2.4760495088926859e-5f);
+				r = fp.sub(fp.mul(r, x2), 1.3888377661039897e-3f);
+				r = fp.add(fp.mul(r, x2), 4.1666638865338612e-2f);
+				r = fp.sub(fp.mul(r, x2), 4.9999999508695869e-1f);
+				r = fp.add(fp.mul(r, x2), 1.0f);
+				return within_half_pi ? r : __uint_as_float(__float_as_uint(r) | 0x80000000u);
+			}
+
+			// rtm::quat_rotation_log(q).xyz (its w is 0): w clamped to [-1, 1] by _mm_min_ss(_mm_max_ss(w, -1), 1) (NaN becomes -1),
+			// xyz * ((1 / sqrt((x x + y y) + z z)) * acos(w)), or xyz itself when the clamped w > 1 - 1e-6
+			__device__ __forceinline__ Vec3<float> quat_rotation_log(const Quat<float>& q)
+			{
+				const Fp<float> fp{};
+				const float lower = q.w > -1.0f ? q.w : -1.0f;
+				const float w = lower < 1.0f ? lower : 1.0f;
+				const float half_angle = rtm_acos(w);
+				const float inv_len = fp.inv_sqrt(fp.add(fp.add(fp.mul(q.x, q.x), fp.mul(q.y, q.y)), fp.mul(q.z, q.z)));
+				const float s = fp.mul(inv_len, half_angle);
+				if (w > 1.0f - 1.0e-6f)
+					return Vec3<float>{ q.x, q.y, q.z };
+				return Vec3<float>{ fp.mul(q.x, s), fp.mul(q.y, s), fp.mul(q.z, s) };
+			}
+
+			// rtm::quat_rotation_exp((v, w)): len = sqrt((x x + y y) + z z), xyz = (v / len) * sin(len), or v itself when len < 1e-6;
+			// w = cos(len)
+			__device__ __forceinline__ Quat<float> quat_rotation_exp(const Vec3<float>& v)
+			{
+				const Fp<float> fp{};
+				const float len = __fsqrt_rn(fp.add(fp.add(fp.mul(v.x, v.x), fp.mul(v.y, v.y)), fp.mul(v.z, v.z)));
+				const float sine = rtm_sin(len);
+				Quat<float> out;
+				out.w = rtm_cos(len);
+				if (len < 1.0e-6f)
+				{
+					out.x = v.x; out.y = v.y; out.z = v.z;
+				}
+				else
+				{
+					out.x = fp.mul(__fdiv_rn(v.x, len), sine);
+					out.y = fp.mul(__fdiv_rn(v.y, len), sine);
+					out.z = fp.mul(__fdiv_rn(v.z, len), sine);
+				}
+				return out;
+			}
+
+			// 2 log(abs(rtm::quat_mul(conj(from), to))).xyz: the scaled angle axis of the rotation that takes `from` to `to` (Hamilton
+			// to from^-1). abs negates all four lanes when w < 0 (an IEEE compare: -0 stays); conj flips the sign bits of x, y and z.
+			__device__ __forceinline__ Vec3<float> scaled_angle_axis_between(const Quat<float>& from, const Quat<float>& to)
+			{
+				const Fp<float> fp{};
+				const Quat<float> conj{ -from.x, -from.y, -from.z, from.w };
+				Quat<float> q = quat_mul(fp, conj, to);
+				if (q.w < 0.0f)
+					q = Quat<float>{ -q.x, -q.y, -q.z, -q.w };
+				const Vec3<float> l = quat_rotation_log(q);
+				return Vec3<float>{ fp.mul(2.0f, l.x), fp.mul(2.0f, l.y), fp.mul(2.0f, l.z) };
+			}
+
+			// One bone's inertialization record entry from its displayed (src) and destination (dst) local rows this frame and the frame
+			// before: rot_x, rot_v, pos_x, pos_v as four float4 (xyz, w = 0) at `entry`, 16 byte aligned. Velocities are backward differences
+			// times inv_dt: (2 log(abs(quat_mul(conj(p_prev), p)))) * inv_dt and (t - t_prev) * inv_dt.
+			__device__ __forceinline__ void capture_inertialization_row(float4* entry, const float4* src_row, const float4* src_prev_row,
+				const float4* dst_row, const float4* dst_prev_row, float inv_dt)
+			{
+				const Fp<float> fp{};
+				const Qvv<float> src = load_qvv_row(src_row), src_prev = load_qvv_row(src_prev_row);
+				const Qvv<float> dst = load_qvv_row(dst_row), dst_prev = load_qvv_row(dst_prev_row);
+				const Vec3<float> rot_x = scaled_angle_axis_between(dst.rotation, src.rotation);
+				const Vec3<float> src_w = scaled_angle_axis_between(src_prev.rotation, src.rotation);
+				const Vec3<float> dst_w = scaled_angle_axis_between(dst_prev.rotation, dst.rotation);
+				entry[0] = make_float4(rot_x.x, rot_x.y, rot_x.z, 0.0f);
+				entry[1] = make_float4(fp.sub(fp.mul(src_w.x, inv_dt), fp.mul(dst_w.x, inv_dt)), fp.sub(fp.mul(src_w.y, inv_dt), fp.mul(dst_w.y, inv_dt)),
+					fp.sub(fp.mul(src_w.z, inv_dt), fp.mul(dst_w.z, inv_dt)), 0.0f);
+				entry[2] = make_float4(fp.sub(src.translation.x, dst.translation.x), fp.sub(src.translation.y, dst.translation.y),
+					fp.sub(src.translation.z, dst.translation.z), 0.0f);
+				const auto velocity = [&](float t, float t_prev) { return fp.mul(fp.sub(t, t_prev), inv_dt); };
+				entry[3] = make_float4(fp.sub(velocity(src.translation.x, src_prev.translation.x), velocity(dst.translation.x, dst_prev.translation.x)),
+					fp.sub(velocity(src.translation.y, src_prev.translation.y), velocity(dst.translation.y, dst_prev.translation.y)),
+					fp.sub(velocity(src.translation.z, src_prev.translation.z), velocity(dst.translation.z, dst_prev.translation.z)), 0.0f);
+			}
+
+			// The critically damped spring of one request, from `elapsed` and `halflife` as given: y = (4 ln 2 / (halflife + 1e-5)) / 2,
+			// e = fast_negexp(y elapsed) = 1 / (((1 + u) + (0.48 u) u) + ((0.235 u) u) u)
+			struct InertializationDecay { float y, e, elapsed; };
+
+			__device__ __forceinline__ InertializationDecay inertialization_decay(float elapsed, float halflife)
+			{
+				const Fp<float> fp{};
+				InertializationDecay d;
+				d.y = fp.mul(__fdiv_rn(2.7725887f, fp.add(halflife, 1.0e-5f)), 0.5f);
+				const float u = fp.mul(d.y, elapsed);
+				d.e = __fdiv_rn(1.0f, fp.add(fp.add(fp.add(1.0f, u), fp.mul(fp.mul(0.48f, u), u)), fp.mul(fp.mul(fp.mul(0.235f, u), u), u)));
+				d.elapsed = elapsed;
+				return d;
+			}
+
+			// x(x0, v0) = e (x0 + (v0 + x0 y) elapsed)
+			__device__ __forceinline__ float decayed(const InertializationDecay& d, float x0, float v0)
+			{
+				const Fp<float> fp{};
+				return fp.mul(d.e, fp.add(x0, fp.mul(fp.add(v0, fp.mul(x0, d.y)), d.elapsed)));
+			}
+
+			// out_row = the destination row `row` with its record entry's offset decayed onto it: rotation quat_mul(dst.q, exp(x(rot_x, rot_v)
+			// * 0.5)) (Hamilton offset dst), translation dst.t + x(pos_x, pos_v), scale dst.s. Rows as apply_additive_row's (QVV48 or
+			// QVV40); out_row may be row.
+			__device__ __forceinline__ void inertialize_row(uint8_t* out_row, const uint8_t* row, const float4* entry, const InertializationDecay& d,
+				bool qvv40)
+			{
+				const Fp<float> fp{};
+				const float4 rot_x = entry[0], rot_v = entry[1], pos_x = entry[2], pos_v = entry[3];
+				const Qvv<float> dst = load_pose_row(row, qvv40);
+				const Vec3<float> half_offset{ fp.mul(decayed(d, rot_x.x, rot_v.x), 0.5f), fp.mul(decayed(d, rot_x.y, rot_v.y), 0.5f),
+					fp.mul(decayed(d, rot_x.z, rot_v.z), 0.5f) };
+				Qvv<float> out;
+				out.rotation = quat_mul(fp, dst.rotation, quat_rotation_exp(half_offset));
+				out.translation = Vec3<float>{ fp.add(dst.translation.x, decayed(d, pos_x.x, pos_v.x)), fp.add(dst.translation.y, decayed(d, pos_x.y, pos_v.y)),
+					fp.add(dst.translation.z, decayed(d, pos_x.z, pos_v.z)) };
+				out.scale = dst.scale;
+				store_pose_row(out_row, out, qvv40);
+			}
 		}
 	}
 }

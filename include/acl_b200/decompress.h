@@ -568,6 +568,44 @@ namespace acl_b200
 			m_device->check(aclb200_search_pose_features(m_device->get(), d_database, num_rows, db_stride, d_row_tags, d_query_vectors, d_queries,
 				num_queries, q_stride, num_dims, d_results, stream), "aclb200_search_pose_features");
 		}
+		// The inertialization record of each transition (aclb200_begin_inertialization): from the displayed QVV48 poses this frame and the
+		// frame before and the destination poses, one frame being 1 / inv_dt seconds; transition j writes record d_record_slots[j], or j.
+		void begin_inertialization(const void* d_src, const void* d_src_prev, const void* d_dst, const void* d_dst_prev, uint64_t num_transitions,
+			uint32_t num_tracks, float inv_dt, void* d_records, const uint32_t* d_record_slots = nullptr, uint64_t pose_stride_bytes = 0,
+			uint64_t record_stride_bytes = 0, void* stream = nullptr)
+		{
+			m_device->check(aclb200_begin_inertialization(m_device->get(), d_src, d_src_prev, d_dst, d_dst_prev, num_transitions, num_tracks,
+				pose_stride_bytes, inv_dt, d_records, record_stride_bytes, d_record_slots, stream), "aclb200_begin_inertialization");
+		}
+		// Each QVV48 pose with its record's offset decayed onto it (aclb200_inertialize_poses); d_out may be d_poses
+		void inertialize_poses(const void* d_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks,
+			const aclb200_inertialization* d_inertializations, const void* d_records, uint64_t num_records, uint64_t pose_stride_bytes = 0,
+			uint64_t record_stride_bytes = 0, void* stream = nullptr)
+		{
+			m_device->check(aclb200_inertialize_poses(m_device->get(), d_poses, d_out, num_poses, num_tracks, pose_stride_bytes, d_inertializations,
+				d_records, num_records, record_stride_bytes, stream), "aclb200_inertialize_poses");
+		}
+		// Decode and inertialize in one launch (aclb200_decompress_tracks_inertialized): local rows without parents, object space rows of
+		// `object_kind` with them; ACLB200_NO_INERTIALIZATION requests as the plain decodes write them
+		void decompress_tracks_inertialized(const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const void* d_records, uint64_t num_records, void* d_out, uint64_t record_stride_bytes = 0, const uint32_t* d_parent_indices = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr,
+			void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_inertialized(m_device->get(), m_clipset, d_requests, num_requests, &options, d_records,
+				num_records, record_stride_bytes, d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream),
+				"aclb200_decompress_tracks_inertialized");
+		}
+		// the same as skinning rows (aclb200_decompress_tracks_inertialized_skinning)
+		void decompress_tracks_inertialized_skinning(const aclb200_inertialized_request* d_requests, uint32_t num_requests,
+			const aclb200_options& options, const void* d_records, uint64_t num_records, const uint32_t* d_parent_indices, const float* d_inverse_bind,
+			void* d_out, uint64_t record_stride_bytes = 0, const uint32_t* d_skeleton_offsets = nullptr, uint32_t* d_out_flags = nullptr,
+			void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_inertialized_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, d_records,
+				num_records, record_stride_bytes, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream),
+				"aclb200_decompress_tracks_inertialized_skinning");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

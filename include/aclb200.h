@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 15
+#define ACLB200_VERSION_MINOR 16
 
 typedef enum aclb200_status
 {
@@ -855,6 +855,102 @@ typedef struct aclb200_search_result
 ACLB200_API aclb200_status aclb200_search_pose_features(aclb200_context* context, const float* d_database, uint64_t num_rows, uint64_t db_stride,
 	const uint32_t* d_row_tags, const float* d_query_vectors, const aclb200_search_query* d_queries, uint32_t num_queries, uint64_t q_stride,
 	uint32_t num_dims, aclb200_search_result* d_results, void* stream);
+
+/* Inertialization: hiding the jump when a character changes clips (a motion matching search result, a state change) without a crossfade.
+ * At the jump, aclb200_begin_inertialization records per bone the offset from the pose the character displayed to the destination pose,
+ * with the offset's velocity. From then on only the destination clip is decoded, and aclb200_inertialize_poses adds the offset as a
+ * critically damped spring decays it to zero. Jumps chain: the next capture starts from the displayed pose, which holds the offset.
+ *
+ * Notation: quat_mul(a, b) is rtm's (apply a, then b: the Hamilton product b a); conj(q) negates x, y and z; abs(q) negates all four lanes
+ * when q.w < 0.0f (an IEEE compare: -0 is kept); log and exp are rtm::quat_rotation_log and rtm::quat_rotation_exp (quatf.h:1306-1375) on
+ * their SSE2 paths, with their near identity and near zero selects; the sin, cos and acos inside them are rtm's polynomials. Every
+ * operation is IEEE and unfused: the results are those of the reference's rtm on any CPU, bit for bit.
+ *
+ * The record: per bone one 64 byte entry of four float4, each xyz plus w = 0; a record is num_tracks entries, 16 byte aligned, in device
+ * memory the caller owns. A caller may write entries directly: for example zeroing the root bone's entry when the root moves by
+ * aclb200_extract_root_motion.
+ *   rot_x  rotation offset as a scaled angle axis: 2 log(abs(quat_mul(conj(dst.q), src.q))).xyz (the Hamilton src dst^-1)
+ *   rot_v  angular velocity offset: w(src) - w(dst), w(p) = (2 log(abs(quat_mul(conj(p_prev.q), p.q))).xyz) * inv_dt
+ *   pos_x  translation offset: src.t - dst.t
+ *   pos_v  linear velocity offset: v(src) - v(dst), v(p) = (p.t - p_prev.t) * inv_dt
+ * Scale is not inertialized (the output takes the destination's scale), so an entry is 64 bytes rather than 96. */
+#define ACLB200_NO_INERTIALIZATION 0xFFFFFFFFu
+#define ACLB200_INERTIALIZATION_ENTRY_BYTES 64u
+
+/* One pose's decay: the record it reads (ACLB200_NO_INERTIALIZATION: none), the seconds since its capture and the spring's halflife in
+ * seconds, both used as given (no clamp). 12 bytes, 4 byte aligned. */
+typedef struct aclb200_inertialization
+{
+	uint32_t record;
+	float    elapsed;
+	float    halflife;
+} aclb200_inertialization;
+
+/* The capture: transition j reads four QVV48 local poses of one skeleton (rtm::qvvf rows, 48 byte bones, 16 byte aligned, pose j of each
+ * buffer at j * pose_stride_bytes, 0 = num_tracks * 48): the displayed pose this frame (d_src) and the frame before (d_src_prev), and the
+ * destination pose this frame (d_dst) and the frame before (d_dst_prev), one frame being 1 / inv_dt seconds. It writes the num_tracks
+ * entries of the record at d_records + slot * record_stride_bytes (0 = num_tracks * 64), slot = d_record_slots[j] (device
+ * uint32[num_transitions]) or j when d_record_slots is NULL. Slots are the caller's to keep in range and distinct.
+ * The displayed poses are what the character showed: its current clip decoded at both times with aclb200_inertialize_poses applied with
+ * its current record (or none). The destination poses come from one aclb200_decompress_tracks launch with two requests per transition.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: NULL or misaligned poses or records with num_transitions > 0, a record
+ * stride below num_tracks * 64 or not a multiple of 16, a slot list not 4 byte aligned, an inv_dt that is zero or not finite. */
+ACLB200_API aclb200_status aclb200_begin_inertialization(aclb200_context* context, const void* d_src, const void* d_src_prev, const void* d_dst,
+	const void* d_dst_prev, uint64_t num_transitions, uint32_t num_tracks, uint64_t pose_stride_bytes, float inv_dt, void* d_records,
+	uint64_t record_stride_bytes, const uint32_t* d_record_slots, void* stream);
+
+/* The apply, on num_poses QVV48 poses already on the device (a decode, a blend, a layer stack; pose p at p * pose_stride_bytes in d_poses
+ * and d_out, 0 = num_tracks * 48). Pose p takes d_inertializations[p] (device) and, unless its record is ACLB200_NO_INERTIALIZATION, the
+ * record at d_records + record * record_stride_bytes (0 = num_tracks * 64). Per pose, from its elapsed and halflife:
+ *     y = (2.7725887f / (halflife + 1e-5f)) * 0.5f;   u = y * elapsed
+ *     e = 1.0f / (((1.0f + u) + (0.48f * u) * u) + ((0.235f * u) * u) * u)
+ *     x(x0, v0) = e * (x0 + (v0 + x0 * y) * elapsed)          per component, in this order
+ * and per bone: rotation quat_mul(dst.q, exp(x(rot_x, rot_v) * 0.5f)) (the Hamilton offset dst), translation dst.t + x(pos_x, pos_v),
+ * scale dst.s; the translation and scale w lanes are written as 0. Nothing is normalised beyond what rtm's functions do.
+ * A pose whose record is ACLB200_NO_INERTIALIZATION is copied unchanged; a pose whose record is >= num_records is not written. d_out may
+ * be d_poses. A record with fewer entries than num_tracks is the caller's error, as for skeleton offsets.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: NULL or misaligned poses, NULL or misaligned (4 byte) d_inertializations
+ * with num_poses > 0, NULL or misaligned (16 byte) d_records with num_records > 0, a record stride below num_tracks * 64 or not a
+ * multiple of 16, num_records >= 2^32 - 1. */
+ACLB200_API aclb200_status aclb200_inertialize_poses(aclb200_context* context, const void* d_poses, void* d_out, uint64_t num_poses,
+	uint32_t num_tracks, uint64_t pose_stride_bytes, const aclb200_inertialization* d_inertializations, const void* d_records,
+	uint64_t num_records, uint64_t record_stride_bytes, void* stream);
+
+/* One request of the inertialized decode: the pose to decode and its inertialization. 20 bytes, 4 byte aligned. */
+typedef struct aclb200_inertialized_request
+{
+	aclb200_request         pose;
+	aclb200_inertialization inertialization;
+} aclb200_inertialized_request;
+
+/* The decode and the apply in one launch, the per-frame call of characters in transition: request r is decoded as aclb200_decompress_tracks
+ * decodes its pose, then, before the rows leave shared memory, the record's offset is decayed onto them exactly as aclb200_inertialize_poses
+ * computes it (QVV48 and QVV40 rows). With parents (d_parent_indices, d_skeleton_offsets and object_kind as aclb200_decompress_tracks_blend)
+ * the inertialized local pose is then taken to object space, as qvvf or 3x4 matrix rows; without them the rows stay local, in
+ * options->output_layout. Records at d_records + record * record_stride_bytes (0 = max_tracks * 64), 16 byte aligned.
+ *   record == ACLB200_NO_INERTIALIZATION   the request reads no record: its rows are byte for byte those of aclb200_decompress_tracks (no
+ *                                          parents), aclb200_decompress_tracks_object_space or _skinning for the same request and options,
+ *                                          so characters not in transition share the launch at no extra traffic
+ *   record >= num_records, invalid clip     nothing is written for the request
+ * A record with fewer entries than the clip's tracks is the caller's error, as for skeleton offsets. d_out_flags as the object space
+ * decode; the inertialization raises no flags. ACLB200_MATH_FAST is accepted and runs the exact decode, as in every composed mode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: the refusals of aclb200_decompress_tracks_blend (skip masks, a `skipped`
+ * default mode, a scalar clip set, alignment, an unknown object_kind, QVV40 with parents), a record stride below max_tracks * 64 or not a
+ * multiple of 16, NULL or misaligned d_records with num_records > 0, num_records >= 2^32 - 1, NULL requests or output with a count above 0.
+ * ACLB200_ERR_UNSUPPORTED when one pose does not fit in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_inertialized(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The skinning rows of the inertialized pose: aclb200_decompress_tracks_inertialized through the matrix walk and the skinning step of
+ * aclb200_decompress_tracks_skinning (parents and inverse binds required). */
+ACLB200_API aclb200_status aclb200_decompress_tracks_inertialized_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
 
 /* The skinning rows of aclb200_decompress_tracks_skinning for poses already on the device (the end of an aclb200_blend_poses chain, of
  * aclb200_apply_additive_to_base): num_poses poses of rtm::qvvf rows of one skeleton (48 byte bones, 16 byte aligned, pose p at
