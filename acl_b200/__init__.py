@@ -24,4 +24,6 @@ from .api import (  # noqa: F401
     FEATURE_POSITION, FEATURE_DIRECTION, FEATURE_VELOCITY, MAX_FEATURE_DIMS, NO_ROW, FEATURE_TERM_DTYPE, SEARCH_QUERY_DTYPE,
     SEARCH_RESULT_DTYPE, make_feature_terms, feature_term_dims, make_search_queries,
     NO_INERTIALIZATION, INERTIALIZATION_DTYPE, make_inertializations, INERTIALIZED_REQUEST_DTYPE, make_inertialized_requests,
+    MIRROR_X, MIRROR_Y, MIRROR_Z, ERROR_FLAG_INVALID_MIRROR, MIRROR_ENTRY_DTYPE, MIRRORED_REQUEST_DTYPE, make_mirrored_requests, mirror_table,
+    mirror_rows_table,
 )

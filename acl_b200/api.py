@@ -182,6 +182,9 @@ def _lib():
         l.aclb200_inertialize_poses.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, u64, u64, vp]
         l.aclb200_decompress_tracks_inertialized.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u64, u64, vp, vp, u32, vp, vp, vp]
         l.aclb200_decompress_tracks_inertialized_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u64, u64, vp, vp, vp, vp, vp, vp]
+        l.aclb200_mirror_poses.argtypes = [vp, vp, vp, u64, u32, u64, vp, vp, u32, vp, vp]
+        l.aclb200_decompress_tracks_mirrored.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, vp, vp, u32, vp, vp, vp]
+        l.aclb200_decompress_tracks_mirrored_skinning.argtypes = [vp, vp, vp, u32, C.POINTER(Options), vp, u32, vp, vp, vp, vp, vp, vp]
         l.aclb200_upload_database.argtypes = [vp, vp, u32, u32, C.POINTER(vp)]
         l.aclb200_release_database.argtypes = [vp, vp]
         l.aclb200_release_database.restype = None
@@ -215,7 +218,8 @@ def exported_symbols() -> list[str]:
         "aclb200_decompress_tracks_layered_masked", "aclb200_decompress_tracks_layered_masked_skinning", "aclb200_decompress_bones",
         "aclb200_extract_root_motion", "aclb200_extract_pose_features", "aclb200_pack_pose_features", "aclb200_search_pose_features",
         "aclb200_begin_inertialization", "aclb200_inertialize_poses", "aclb200_decompress_tracks_inertialized",
-        "aclb200_decompress_tracks_inertialized_skinning",
+        "aclb200_decompress_tracks_inertialized_skinning", "aclb200_mirror_poses", "aclb200_decompress_tracks_mirrored",
+        "aclb200_decompress_tracks_mirrored_skinning",
     ]
 
 
@@ -282,6 +286,12 @@ NO_INERTIALIZATION = 0xFFFFFFFF  # an inertialization that reads no record
 INERTIALIZATION_DTYPE = np.dtype([("record", np.uint32), ("elapsed", np.float32), ("halflife", np.float32)])
 INERTIALIZED_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("record", np.uint32), ("elapsed", np.float32),
                                        ("halflife", np.float32)])
+
+
+MIRROR_X, MIRROR_Y, MIRROR_Z = 0, 1, 2  # the normal of the mirror plane
+ERROR_FLAG_INVALID_MIRROR = 8  # a mirror table entry without a partner row
+MIRROR_ENTRY_DTYPE = np.dtype([("pre", np.float32, 4), ("post", np.float32, 4), ("mirror", np.uint32), ("reserved", np.uint32, 3)])
+MIRRORED_REQUEST_DTYPE = np.dtype([("clip", np.uint32), ("sample_time", np.float32), ("mirrored", np.uint32)])
 
 
 def make_layers(clips, times, ops, weights) -> np.ndarray:
@@ -358,6 +368,88 @@ def make_inertialized_requests(clips, times, records, elapsed, halflife) -> np.n
     for name, value in zip(INERTIALIZED_REQUEST_DTYPE.names, fields):
         out[name] = value
     return out.reshape(-1)
+
+
+def make_mirrored_requests(clips, times, mirrored) -> np.ndarray:
+    """(clip index, sample time, 0 plain / 1 mirrored) arrays, or anything that broadcasts to one shape -> aclb200_mirrored_request[]"""
+    fields = np.broadcast_arrays(np.asarray(clips, dtype=np.uint32), np.asarray(times, dtype=np.float32), np.asarray(mirrored, dtype=np.uint32))
+    out = np.empty(fields[0].shape, dtype=MIRRORED_REQUEST_DTYPE)
+    for name, value in zip(MIRRORED_REQUEST_DTYPE.names, fields):
+        out[name] = value
+    return out.reshape(-1)
+
+
+def _quat_mul64(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """rtm's quat_mul(a, b) (apply a, then b: the Hamilton product b a) on float64 xyzw quaternions, broadcasting"""
+    ax, ay, az, aw = np.moveaxis(a, -1, 0)
+    bx, by, bz, bw = np.moveaxis(b, -1, 0)
+    return np.stack([bw * ax + bx * aw + by * az - bz * ay,
+                     bw * ay - bx * az + by * aw + bz * ax,
+                     bw * az + bx * ay - by * ax + bz * aw,
+                     bw * aw - bx * ax - by * ay - bz * az], axis=-1)
+
+
+def _conj64(q: np.ndarray) -> np.ndarray:
+    return q * np.array([-1.0, -1.0, -1.0, 1.0])
+
+
+def _reflect_q64(q: np.ndarray, axis: int) -> np.ndarray:
+    sign = -np.ones(4)
+    sign[axis] = 1.0
+    sign[3] = 1.0
+    return q * sign
+
+
+def mirror_table(parents, mirror_bones, bind_object_rotations, axis: int) -> np.ndarray:
+    """A skeleton's mirror table for local pose rows (MIRROR_ENTRY_DTYPE[num_bones]), from its parents (0xFFFFFFFF for roots),
+    each bone's mirror bone and its bind pose's object space rotations (float [num_bones][4], xyzw). Bone b's correction is
+    C_b = quat_mul(Q_b, conj(reflect_q(Q_m(b)))) in float64, normalised, then rounded to float32; pre_b = C_b and post_b =
+    conj(C_parent(b)) (identity for roots), so that mirroring the bind pose returns it. Raises ValueError unless mirror_bones is an
+    involution (m(m(b)) == b) and the hierarchy is symmetric (parent(m(b)) == m(parent(b)), roots mirror to roots)."""
+    parents = np.asarray(parents, dtype=np.int64).reshape(-1)
+    mirror = np.asarray(mirror_bones, dtype=np.int64).reshape(-1)
+    q = np.asarray(bind_object_rotations, dtype=np.float64).reshape(-1, 4)
+    n = parents.shape[0]
+    if axis not in (MIRROR_X, MIRROR_Y, MIRROR_Z):
+        raise ValueError("axis must be MIRROR_X, MIRROR_Y or MIRROR_Z")
+    if mirror.shape[0] != n or q.shape[0] != n:
+        raise ValueError("parents, mirror_bones and bind_object_rotations need one entry per bone")
+    if ((mirror < 0) | (mirror >= n)).any() or (mirror[mirror] != np.arange(n)).any():
+        raise ValueError("mirror_bones is not an involution over the skeleton's bones")
+    is_root = (parents < 0) | (parents >= n)
+    for b in range(n):
+        m = mirror[b]
+        if is_root[b] != is_root[m] or (not is_root[b] and parents[m] != mirror[parents[b]]):
+            raise ValueError(f"the hierarchy is not symmetric: parent(m({b})) != m(parent({b}))")
+    c = _quat_mul64(q, _conj64(_reflect_q64(q[mirror], axis)))
+    c = (c / np.linalg.norm(c, axis=-1, keepdims=True)).astype(np.float32)
+    table = np.zeros(n, dtype=MIRROR_ENTRY_DTYPE)
+    table["pre"] = c
+    post = np.tile(np.array([0, 0, 0, 1], np.float32), (n, 1))
+    post[~is_root] = _conj64(c[parents[~is_root]].astype(np.float64)).astype(np.float32)
+    table["post"] = post
+    table["mirror"] = mirror.astype(np.uint32)
+    return table
+
+
+def mirror_rows_table(table: np.ndarray, bones, frame_bone: int) -> np.ndarray:
+    """The mirror table of rows that hold the listed bones relative to frame_bone, from a skeleton's table (mirror_table): pose feature
+    rows (bones = a bone list, frame_bone = the root) or root motion rows (bones = [root], frame_bone = root). Row k takes pre = C of
+    bones[k], post = conj(C of frame_bone) and the row whose bone is bones[k]'s mirror bone. Raises ValueError when a listed bone's mirror
+    bone is not listed."""
+    table = np.asarray(table)
+    bones = [int(b) for b in np.asarray(bones).reshape(-1)]
+    row_of = {b: k for k, b in enumerate(bones)}
+    out = np.zeros(len(bones), dtype=MIRROR_ENTRY_DTYPE)
+    post = _conj64(table["pre"][frame_bone].astype(np.float64)).astype(np.float32)
+    for k, b in enumerate(bones):
+        m = int(table["mirror"][b])
+        if m not in row_of:
+            raise ValueError(f"bone {b}'s mirror bone {m} is not among the rows")
+        out["pre"][k] = table["pre"][b]
+        out["post"][k] = post
+        out["mirror"][k] = row_of[m]
+    return out
 
 
 def make_search_queries(tag_masks=0xFFFFFFFF, exclude_begin=0, exclude_end=0) -> np.ndarray:
@@ -850,6 +942,35 @@ class Context:
                                                                            record_stride_bytes, _device_ptr(d_parent_indices),
                                                                            _device_ptr(d_skeleton_offsets), _device_ptr(d_inverse_bind),
                                                                            _device_ptr(d_out), _device_ptr(d_out_flags), _stream_ptr(stream)))
+
+    def mirror_poses(self, d_poses, d_out, num_poses: int, num_rows: int, d_table, axis: int, d_mirrored=None, pose_stride_bytes: int = 0,
+                     d_out_flags=None, stream=None) -> None:
+        """Each QVV48 pose of num_rows rows mirrored with d_table (MIRROR_ENTRY_DTYPE bytes, one per row) across the plane normal to
+        `axis`. d_mirrored (uint32 per pose, optional): 0 copies the pose, 1 mirrors it, anything else leaves it unwritten; without it
+        every pose is mirrored. d_out may be d_poses."""
+        self._check(_lib().aclb200_mirror_poses(self._handle, _device_ptr(d_poses), _device_ptr(d_out), num_poses, num_rows, pose_stride_bytes,
+                                                _device_ptr(d_mirrored), _device_ptr(d_table), axis, _device_ptr(d_out_flags),
+                                                _stream_ptr(stream)))
+
+    def decompress_tracks_mirrored(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_out, d_mirror_table, axis: int,
+                                   d_parent_indices=None, kind: int = 0, d_skeleton_offsets=None, d_out_flags=None, stream=None) -> None:
+        """num_requests mirrored requests (make_mirrored_requests): each pose decoded, then mirrored in the same launch when its request
+        says 1 (0: the plain decode's rows; anything else: nothing written). Clip c's table is at d_mirror_table + d_skeleton_offsets[c]
+        entries. With d_parent_indices the pose leaves in object space as `kind` rows (OBJECT_*); without, in options.output_layout."""
+        self._check(_lib().aclb200_decompress_tracks_mirrored(self._handle, clipset._handle, _device_ptr(d_requests), num_requests, C.byref(options),
+                                                              _device_ptr(d_mirror_table), axis, _device_ptr(d_parent_indices),
+                                                              _device_ptr(d_skeleton_offsets), kind, _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                              _stream_ptr(stream)))
+
+    def decompress_tracks_mirrored_skinning(self, clipset: ClipSet, d_requests, num_requests: int, options: Options, d_parent_indices,
+                                            d_inverse_bind, d_out, d_mirror_table, axis: int, d_skeleton_offsets=None, d_out_flags=None,
+                                            stream=None) -> None:
+        """decompress_tracks_mirrored's poses as skinning rows, with the clip's skeleton and inverse binds."""
+        self._check(_lib().aclb200_decompress_tracks_mirrored_skinning(self._handle, clipset._handle, _device_ptr(d_requests), num_requests,
+                                                                       C.byref(options), _device_ptr(d_mirror_table), axis,
+                                                                       _device_ptr(d_parent_indices), _device_ptr(d_skeleton_offsets),
+                                                                       _device_ptr(d_inverse_bind), _device_ptr(d_out), _device_ptr(d_out_flags),
+                                                                       _stream_ptr(stream)))
 
     # ---- host buffers in, host buffers out (the call the C++ header shim uses) ----
     def decompress_tracks_host(self, clipset: ClipSet, requests: np.ndarray, options: Options, out: np.ndarray) -> np.ndarray:

@@ -46,6 +46,9 @@ namespace aclb200
 			const void* d_records;
 			uint64_t record_stride;					// resolved by check_records (0 = max_tracks * 64)
 			uint64_t num_records;
+			// mirror: the table of skeleton 0 and the axis (every field 0 in the other modes)
+			const aclb200_mirror_entry* d_mirror_table;
+			uint32_t mirror_axis;
 		};
 		const char* const k_pose_unfit = ": one pose does not fit in a block's shared memory";
 		const char* const k_pair_unfit = ": the two poses of a pair do not fit in a block's shared memory";
@@ -243,6 +246,16 @@ namespace aclb200
 		return ACLB200_OK;
 	}
 
+	// mirroring: a known axis, and a 16 byte aligned table wherever there is work to do
+	aclb200_status check_mirror(aclb200_context* context, const aclb200_mirror_entry* d_table, uint32_t axis, bool work, const char* what)
+	{
+		if (axis > ACLB200_MIRROR_Z)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": axis must be ACLB200_MIRROR_X, _Y or _Z");
+		if (work && (d_table == nullptr || (reinterpret_cast<uintptr_t>(d_table) % 16) != 0))
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, std::string(what) + ": the mirror table is 48 byte entries, 16 byte aligned, never NULL");
+		return ACLB200_OK;
+	}
+
 	aclb200_status check_inverse_binds(aclb200_context* context, const float* d_inverse_bind, const char* what)
 	{
 		if (d_inverse_bind == nullptr || (reinterpret_cast<uintptr_t>(d_inverse_bind) % 16) != 0)
@@ -338,6 +351,8 @@ namespace aclb200
 			params.records = static_cast<const uint8_t*>(composed.d_records);
 			params.record_stride = composed.record_stride;
 			params.num_records = uint32_t(composed.num_records);
+			params.mirror_table = composed.d_mirror_table;
+			params.mirror_axis = composed.mirror_axis;
 			cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
 			return launch_clearing_flags(context, d_out_flags, cuda_stream, entry.c_str(), entry.c_str(),
 				[&] { return launch_transform_decompress_tracks(params, composed.compose, params.db_tiers != nullptr, cuda_stream); });
@@ -437,6 +452,27 @@ namespace aclb200
 			return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
 				skinning, d_inverse_bind, d_out, d_out_flags, stream);
 		}
+
+		// the mirrored decode and its _skinning sibling: the axis and table checks, then the composed path (requests are 12 byte records)
+		aclb200_status decompress_mirrored(aclb200_context* context, const aclb200_clipset* clipset, const aclb200_mirrored_request* d_requests,
+			uint32_t num_requests, const aclb200_options* options, const aclb200_mirror_entry* d_mirror_table, uint32_t axis,
+			const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind, bool skinning, const float* d_inverse_bind,
+			void* d_out, uint32_t* d_out_flags, void* stream)
+		{
+			const char* what = skinning ? "decompress_tracks_mirrored_skinning" : "decompress_tracks_mirrored";
+			if (context == nullptr || clipset == nullptr)
+				return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "null context / clipset / options");
+			const aclb200_status status = check_mirror(context, d_mirror_table, axis, num_requests != 0, what);
+			if (status != ACLB200_OK)
+				return status;
+			static_assert(sizeof(aclb200_mirrored_request) == 12 && offsetof(aclb200_mirrored_request, mirrored) == 8,
+				"a mirrored request is a request and its flag, three words");
+			Composed composed = { what, k_pose_unfit, k_compose_mirror, 1 };
+			composed.d_mirror_table = d_mirror_table;
+			composed.mirror_axis = axis;
+			return decompress_composed(context, clipset, d_requests, num_requests, options, composed, d_parent_indices, d_skeleton_offsets, object_kind,
+				skinning, d_inverse_bind, d_out, d_out_flags, stream);
+		}
 	}
 }
 
@@ -446,7 +482,7 @@ extern "C"
 {
 	const char* aclb200_version_string(void)
 	{
-		return "aclb200 0.16 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
+		return "aclb200 0.17 (sm_90a; ACL compressed_tracks v02_00_00..v02_01_00)";
 	}
 
 	const char* aclb200_status_string(aclb200_status status)
@@ -1141,6 +1177,61 @@ extern "C"
 	{
 		return decompress_inertialized(context, clipset, d_requests, num_requests, options, d_records, num_records, record_stride_bytes,
 			d_parent_indices, d_skeleton_offsets, ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_mirror_poses(aclb200_context* context, const void* d_poses, void* d_out, uint64_t num_poses, uint32_t num_rows,
+		uint64_t pose_stride_bytes, const uint32_t* d_mirrored, const aclb200_mirror_entry* d_table, uint32_t axis, uint32_t* d_out_flags,
+		void* stream)
+	{
+		if (context == nullptr)
+			return ACLB200_ERR_INVALID_ARGUMENT;
+		const bool work = num_poses != 0 && num_rows != 0;
+		aclb200_status status = check_mirror(context, d_table, axis, work, "mirror_poses");
+		if (status != ACLB200_OK)
+			return status;
+		if (!work)
+			return ACLB200_OK;
+		if (d_poses == nullptr || d_out == nullptr)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "mirror_poses: null pose pointer");
+		if (reinterpret_cast<uintptr_t>(d_mirrored) % 4 != 0)
+			return set_error(context, ACLB200_ERR_INVALID_ARGUMENT, "mirror_poses: d_mirrored must be 4 byte aligned");
+		uint64_t stride = pose_stride_bytes;
+		status = check_qvvf_rows(context, { d_poses, d_out }, num_rows, stride, "mirror_poses");
+		if (status != ACLB200_OK)
+			return status;
+		MirrorApply apply = {};
+		apply.poses = static_cast<const uint8_t*>(d_poses);
+		apply.out = static_cast<uint8_t*>(d_out);
+		apply.mirrored = d_mirrored;
+		apply.table = d_table;
+		apply.flags = d_out_flags;
+		apply.num_poses = num_poses;
+		apply.pose_stride = stride;
+		apply.num_rows = num_rows;
+		apply.axis = axis;
+		cudaStream_t cuda_stream = static_cast<cudaStream_t>(stream);
+		return launch_clearing_flags(context, d_out_flags, cuda_stream, "mirror_poses", "mirror_poses",
+			[&] { return launch_mirror_poses(apply, context->num_sms, cuda_stream); });
+	}
+
+	aclb200_status aclb200_decompress_tracks_mirrored(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const aclb200_mirror_entry* d_mirror_table, uint32_t axis,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		return decompress_mirrored(context, clipset, d_requests, num_requests, options, d_mirror_table, axis, d_parent_indices, d_skeleton_offsets,
+			object_kind, false, nullptr, d_out, d_out_flags, stream);
+	}
+
+	aclb200_status aclb200_decompress_tracks_mirrored_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+		const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+		const aclb200_mirror_entry* d_mirror_table, uint32_t axis,
+		const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+		void* d_out, uint32_t* d_out_flags, void* stream)
+	{
+		return decompress_mirrored(context, clipset, d_requests, num_requests, options, d_mirror_table, axis, d_parent_indices, d_skeleton_offsets,
+			ACLB200_OBJECT_MATRIX3X4F, true, d_inverse_bind, d_out, d_out_flags, stream);
 	}
 
 	aclb200_status aclb200_local_to_skinning(aclb200_context* context, const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks,

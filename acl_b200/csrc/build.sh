@@ -10,5 +10,5 @@ NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
   --fmad=false -Xptxas -v \
   -Xcompiler -fPIC,-fvisibility=hidden,-Wall -shared -cudart static \
   -o "$OUT" \
-  "$HERE/kernels.cu" "$HERE/pipeline.cu" "$HERE/bones.cu" "$HERE/root_motion.cu" "$HERE/features.cu" "$HERE/feature_search.cu" "$HERE/inertialization.cu" "$HERE/error_metric.cu" "$HERE/clipset.cpp" "$HERE/database.cpp" "$HERE/api.cpp" "$@"
+  "$HERE/kernels.cu" "$HERE/pipeline.cu" "$HERE/bones.cu" "$HERE/root_motion.cu" "$HERE/features.cu" "$HERE/feature_search.cu" "$HERE/inertialization.cu" "$HERE/mirror.cu" "$HERE/error_metric.cu" "$HERE/clipset.cpp" "$HERE/database.cpp" "$HERE/api.cpp" "$@"
 echo "built $OUT"

@@ -201,6 +201,10 @@ namespace aclb200
 		const uint8_t* records;						// record r at records + r * record_stride, 64 bytes per bone
 		uint64_t record_stride;
 		uint32_t num_records;						// < 2^32 - 1
+		// the mirrored decode (aclb200_decompress_tracks_mirrored, k_compose_mirror): `requests` holds 12 byte aclb200_mirrored_request
+		// records; clip c's table at mirror_table + skeleton_offsets[c]
+		const aclb200_mirror_entry* mirror_table;
+		uint32_t mirror_axis;						// ACLB200_MIRROR_*
 	};
 
 	// The bone query (aclb200_decompress_bones, bones.cu): the lists, the skeletons and the launch's shared memory carve-up. A kernel
@@ -315,14 +319,28 @@ namespace aclb200
 		uint32_t num_tracks;
 	};
 
+	// The pose mirror (aclb200_mirror_poses, mirror.cu): pose p at p * pose_stride in poses and out, row i mirrored with table[i]
+	struct MirrorApply
+	{
+		const uint8_t* poses;
+		uint8_t* out;
+		const uint32_t* mirrored;				// [num_poses] 0 copy, 1 mirror, other: not written; NULL: every pose mirrored
+		const aclb200_mirror_entry* table;
+		uint32_t* flags;
+		uint64_t num_poses;
+		uint64_t pose_stride;
+		uint32_t num_rows;
+		uint32_t axis;
+	};
+
 	// What transform_decompress_tracks_kernel makes of its poses before they leave. local: the decoded poses (aclb200_decompress_tracks).
 	// object: taken to object space (aclb200_decompress_tracks_object_space). additive, blend: pair r is requests 2r and 2r + 1, combined
 	// into output r (aclb200_decompress_tracks_additive / _blend). layers: stack r is requests r L .. r L + L - 1, folded into output r
 	// (aclb200_decompress_tracks_layered). layers_masked: the layers mode with bone masks and weighted ADDITIVE layers
 	// (aclb200_decompress_tracks_layered_masked). inertialize: each request's pose with its inertialization record's offset decayed onto
-	// it (aclb200_decompress_tracks_inertialized).
+	// it (aclb200_decompress_tracks_inertialized). mirror: each request's pose, mirrored when its request asks (aclb200_decompress_tracks_mirrored).
 	enum : uint32_t { k_compose_local = 0, k_compose_object = 1, k_compose_additive = 2, k_compose_blend = 3, k_compose_layers = 4,
-		k_compose_layers_masked = 5, k_compose_inertialize = 6, k_compose_count = 7 };
+		k_compose_layers_masked = 5, k_compose_inertialize = 6, k_compose_mirror = 7, k_compose_count = 8 };
 
 	// the deepest layer stack of aclb200_decompress_tracks_layered
 	constexpr uint32_t k_max_layers = 8;
@@ -378,6 +396,8 @@ namespace aclb200
 	// inertialization.cu: the capture and the apply, one thread per (pose, bone)
 	cudaError_t launch_begin_inertialization(const InertializationCapture& capture, int num_sms, cudaStream_t stream);
 	cudaError_t launch_inertialize_poses(const InertializationApply& apply, int num_sms, cudaStream_t stream);
+	// mirror.cu: one thread per (pose, partner pair)
+	cudaError_t launch_mirror_poses(const MirrorApply& apply, int num_sms, cudaStream_t stream);
 	// error_metric.cu
 	cudaError_t configure_error_kernels(int optin_limit);
 	// pipeline.cu

@@ -59,6 +59,14 @@ namespace aclb200
 			uint32_t unused;
 		};
 		static_assert(sizeof(InertializationSlot) == sizeof(LayerSlot), "an inertialization slot takes a layer slot's place");
+
+		// The mirrored decode keeps each request's `mirrored` word in the same 16 byte slot
+		struct alignas(16) MirrorSlot
+		{
+			uint32_t mirrored;
+			uint32_t unused[3];
+		};
+		static_assert(sizeof(MirrorSlot) == sizeof(LayerSlot), "a mirror slot takes a layer slot's place");
 		constexpr uint32_t k_layer_base = 3, k_layer_unknown = 4, k_no_base = 0xFFFFFFFFu;
 		constexpr uint32_t k_layer_op_mask = (1u << k_layer_op_bits) - 1;
 
@@ -98,6 +106,9 @@ namespace aclb200
 		//             records; a request whose record is at or above p.num_records is not sought (it writes nothing). Phase 4c decays the
 		//             record's offset onto each bone's row in place (obj::inertialize_row); ACLB200_NO_INERTIALIZATION rows are left as
 		//             decoded. Phases 4b and 5 then run as for the object mode when parents are given, and store local rows without them.
+		//             k_compose_mirror (aclb200_decompress_tracks_mirrored): requests are 12 byte aclb200_mirrored_request records; a request
+		//             whose `mirrored` is neither 0 nor 1 is not sought (it writes nothing). Phase 4c mirrors the rows of each request with
+		//             mirrored == 1 in place, one thread per partner pair (obj::mirror_row); phases 4b and 5 as in the inertialized mode.
 		template<int NORM, bool PER_TRACK, bool STAGED, bool OUT_STAGED, bool DB, uint32_t COMPOSE>
 		__global__ void __launch_bounds__(k_threads_per_block)
 		transform_decompress_tracks_kernel(const DecodeParams p)
@@ -106,6 +117,7 @@ namespace aclb200
 			constexpr bool MASKED = COMPOSE == k_compose_layers_masked;
 			constexpr bool LAYERED = COMPOSE == k_compose_layers || MASKED;
 			constexpr bool INERT = COMPOSE == k_compose_inertialize;
+			constexpr bool MIRROR = COMPOSE == k_compose_mirror;
 			// MASKED: a layer slot's op carries the layer's mask index above its low k_layer_op_bits
 			auto slot_op = [](uint32_t slot) { return MASKED ? slot & k_layer_op_mask : slot; };
 			static_assert(COMPOSE == k_compose_local || OUT_STAGED, "the composed decodes work on poses assembled in shared memory");
@@ -128,6 +140,7 @@ namespace aclb200
 			if (LAYERED && threadIdx.x == 0)
 				s_layer[0].num_stacks = fast_div(num_requests, p.magic_layers);
 			InertializationSlot* s_inert = reinterpret_cast<InertializationSlot*>(s_layer);
+			MirrorSlot* s_mirror = reinterpret_cast<MirrorSlot*>(s_layer);
 
 			if (STAGED)
 			{
@@ -172,6 +185,16 @@ namespace aclb200
 					if (record == ACLB200_NO_INERTIALIZATION || record < p.num_records)
 						seek_request<DB>(p, aclb200_request{ __ldg(words), __uint_as_float(__ldg(words + 1)) }, first_request + threadIdx.x, rs);
 					s_inert[threadIdx.x] = InertializationSlot{ record, __uint_as_float(__ldg(words + 3)), __uint_as_float(__ldg(words + 4)), 0u };
+				}
+				else if constexpr (MIRROR)
+				{
+					// {clip, sample_time, mirrored}, three words at 4 byte alignment
+					const uint32_t* words = reinterpret_cast<const uint32_t*>(p.requests) + uint64_t(first_request + threadIdx.x) * 3;
+					const uint32_t mirrored = __ldg(words + 2);
+					rs.num_tracks = 0;
+					if (mirrored <= 1u)
+						seek_request<DB>(p, aclb200_request{ __ldg(words), __uint_as_float(__ldg(words + 1)) }, first_request + threadIdx.x, rs);
+					s_mirror[threadIdx.x].mirrored = mirrored;
 				}
 				else
 					seek_transform<DB, RS, PAIRED>(p, first_request + threadIdx.x, rs);
@@ -415,11 +438,42 @@ namespace aclb200
 				}
 			}
 
+			// ---- phase 4c, mirror: one thread per (request, bone) of the mirrored requests; the thread of the lower row of each partner pair
+			// mirrors both rows in place, so no other thread touches them. The clip's table is indexed like its parents ----
+			if constexpr (MIRROR)
+			{
+				__syncthreads();
+				uint32_t flags = 0;
+				const uint32_t num_slots = num_requests * p.max_tracks;
+				for (uint32_t slot = threadIdx.x; slot < num_slots; slot += k_threads_per_block)
+				{
+					const uint32_t local_request = fast_div(slot, p.magic_tracks);
+					const uint32_t bone = slot - local_request * p.max_tracks;
+					const uint32_t num_tracks = s_req[local_request].num_tracks;
+					if (bone >= num_tracks || s_mirror[local_request].mirrored != 1u)
+						continue;
+					const uint32_t skeleton = p.skeleton_offsets != nullptr ? __ldg(p.skeleton_offsets + s_req[local_request].clip) : 0u;
+					const aclb200_mirror_entry* table = p.mirror_table + skeleton;
+					bool invalid = false;
+					const uint32_t partner = obj::mirror_partner(table, bone, num_tracks, invalid);
+					if (invalid)
+						flags |= ACLB200_ERROR_FLAG_INVALID_MIRROR;
+					if (partner < bone)
+						continue;
+					uint8_t* pose = s_out + size_t(local_request) * p.smem_pose_bytes;
+					uint8_t* row = pose + size_t(bone) * p.bone_stride;
+					uint8_t* partner_row = pose + size_t(partner) * p.bone_stride;
+					obj::mirror_row(row, partner_row, row, partner_row, table + bone, table + partner, p.mirror_axis, p.layout == ACLB200_LAYOUT_QVV40);
+				}
+				if (flags != 0 && p.object_flags != nullptr)
+					atomicOr(p.object_flags, flags);
+			}
+
 			// ---- phase 4b: one warp per staged pose walks the clip's skeleton and overwrites the local rows with object rows (PAIRED: the
 			// combined row of each pair, when parents are given) ----
 			if constexpr (COMPOSE != k_compose_local)
 			{
-				if ((!PAIRED && !LAYERED && !INERT) || p.parent_indices != nullptr)
+				if ((!PAIRED && !LAYERED && !INERT && !MIRROR) || p.parent_indices != nullptr)
 				{
 					__syncthreads();
 					uint32_t flags = 0;
@@ -1132,7 +1186,8 @@ namespace aclb200
 		const bool force_output_staging = compose != k_compose_local;
 		const bool pairs = compose == k_compose_additive || compose == k_compose_blend;
 		const bool layers = compose == k_compose_layers || compose == k_compose_layers_masked;
-		const bool slots = layers || compose == k_compose_inertialize;		// a LayerSlot or an InertializationSlot beside each request state
+		// a LayerSlot, an InertializationSlot or a MirrorSlot beside each request state
+		const bool slots = layers || compose == k_compose_inertialize || compose == k_compose_mirror;
 		const uint32_t state_bytes = (database ? uint32_t(sizeof(ReqStateDB)) : uint32_t(sizeof(ReqState))) + (slots ? uint32_t(sizeof(LayerSlot)) : 0u);
 		const uint32_t max_tracks = params.max_tracks == 0 ? 1 : params.max_tracks;
 		const uint32_t budget = uint32_t(max_dynamic_smem > 0 ? max_dynamic_smem : 0);

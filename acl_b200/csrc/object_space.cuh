@@ -885,6 +885,53 @@ namespace aclb200
 				out.scale = dst.scale;
 				store_pose_row(out_row, out, qvv40);
 			}
+
+			// ---- mirroring (aclb200_mirror_poses, the mirrored decode): reflect_q flips the sign bits of the quaternion lanes other than
+			// `axis`, reflect_t the translation lane `axis`; sign bit flips, so -0 / +0 swap and NaN payloads stay ----
+			__device__ __forceinline__ float flip_sign(float v, bool flip)
+			{
+				return __uint_as_float(__float_as_uint(v) ^ (flip ? 0x80000000u : 0u));
+			}
+
+			// row i's partner among n rows: m = table[i].mirror when m < n and table[m].mirror == i, else i itself with invalid set
+			__device__ __forceinline__ uint32_t mirror_partner(const aclb200_mirror_entry* table, uint32_t i, uint32_t n, bool& invalid)
+			{
+				const uint32_t m = __ldg(&table[i].mirror);
+				if (m < n && __ldg(&table[m].mirror) == i)
+					return m;
+				invalid = true;
+				return i;
+			}
+
+			// the mirrored row from the partner's row `src` and this row's entry: rotation quat_mul(quat_mul(pre, reflect_q(q)), post),
+			// translation quat_mul_vector3(reflect_t(t), post), scale copied
+			__device__ __forceinline__ Qvv<float> mirrored_row(const Qvv<float>& src, const aclb200_mirror_entry* entry, uint32_t axis)
+			{
+				const Fp<float> fp{};
+				const float4 pre = __ldg(reinterpret_cast<const float4*>(entry->pre));
+				const float4 post = __ldg(reinterpret_cast<const float4*>(entry->post));
+				const Quat<float> reflected{ flip_sign(src.rotation.x, axis != 0), flip_sign(src.rotation.y, axis != 1),
+					flip_sign(src.rotation.z, axis != 2), src.rotation.w };
+				const Quat<float> post_q{ post.x, post.y, post.z, post.w };
+				Qvv<float> out;
+				out.rotation = quat_mul(fp, quat_mul(fp, Quat<float>{ pre.x, pre.y, pre.z, pre.w }, reflected), post_q);
+				out.translation = quat_mul_vector3(fp, Vec3<float>{ flip_sign(src.translation.x, axis == 0), flip_sign(src.translation.y, axis == 1),
+					flip_sign(src.translation.z, axis == 2) }, post_q);
+				out.scale = src.scale;
+				return out;
+			}
+
+			// A partner pair (row i, row m; the same row for a self partner) read from in_i / in_m and written to out_i / out_m, each from
+			// the other's transform. Rows as apply_additive_row's (QVV48 or QVV40); the outputs may be the inputs.
+			__device__ __forceinline__ void mirror_row(uint8_t* out_i, uint8_t* out_m, const uint8_t* in_i, const uint8_t* in_m,
+				const aclb200_mirror_entry* entry_i, const aclb200_mirror_entry* entry_m, uint32_t axis, bool qvv40)
+			{
+				const Qvv<float> row_i = load_pose_row(in_i, qvv40);
+				const Qvv<float> row_m = load_pose_row(in_m, qvv40);
+				store_pose_row(out_i, mirrored_row(row_m, entry_i, axis), qvv40);
+				if (entry_m != entry_i)
+					store_pose_row(out_m, mirrored_row(row_i, entry_m, axis), qvv40);
+			}
 		}
 	}
 }

@@ -606,6 +606,32 @@ namespace acl_b200
 				num_records, record_stride_bytes, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream),
 				"aclb200_decompress_tracks_inertialized_skinning");
 		}
+		// Each QVV48 pose of num_rows rows mirrored with d_table across the plane normal to `axis` (aclb200_mirror_poses); d_mirrored per
+		// pose: 0 copies, 1 mirrors, other values leave the pose unwritten, NULL mirrors every pose. d_out may be d_poses.
+		void mirror_poses(const void* d_poses, void* d_out, uint64_t num_poses, uint32_t num_rows, const aclb200_mirror_entry* d_table, uint32_t axis,
+			const uint32_t* d_mirrored = nullptr, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_mirror_poses(m_device->get(), d_poses, d_out, num_poses, num_rows, pose_stride_bytes, d_mirrored, d_table, axis,
+				d_out_flags, stream), "aclb200_mirror_poses");
+		}
+		// Decode and mirror in one launch (aclb200_decompress_tracks_mirrored): local rows without parents, object space rows of
+		// `object_kind` with them; requests with mirrored == 0 as the plain decodes write them
+		void decompress_tracks_mirrored(const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const aclb200_mirror_entry* d_mirror_table, uint32_t axis, void* d_out, const uint32_t* d_parent_indices = nullptr,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t object_kind = ACLB200_OBJECT_QVVF, uint32_t* d_out_flags = nullptr,
+			void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_mirrored(m_device->get(), m_clipset, d_requests, num_requests, &options, d_mirror_table, axis,
+				d_parent_indices, d_skeleton_offsets, object_kind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_mirrored");
+		}
+		// the same as skinning rows (aclb200_decompress_tracks_mirrored_skinning)
+		void decompress_tracks_mirrored_skinning(const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options& options,
+			const aclb200_mirror_entry* d_mirror_table, uint32_t axis, const uint32_t* d_parent_indices, const float* d_inverse_bind, void* d_out,
+			const uint32_t* d_skeleton_offsets = nullptr, uint32_t* d_out_flags = nullptr, void* stream = nullptr)
+		{
+			m_device->check(aclb200_decompress_tracks_mirrored_skinning(m_device->get(), m_clipset, d_requests, num_requests, &options, d_mirror_table,
+				axis, d_parent_indices, d_skeleton_offsets, d_inverse_bind, d_out, d_out_flags, stream), "aclb200_decompress_tracks_mirrored_skinning");
+		}
 		// over num_poses QVV48 poses of one skeleton already on the device (aclb200_local_to_skinning); d_out may be d_local_poses
 		void local_to_skinning(const void* d_local_poses, void* d_out, uint64_t num_poses, uint32_t num_tracks, const uint32_t* d_parent_indices,
 			const float* d_inverse_bind, uint64_t pose_stride_bytes = 0, uint32_t* d_out_flags = nullptr, void* stream = nullptr)

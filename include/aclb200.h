@@ -32,7 +32,7 @@ extern "C" {
 #endif
 
 #define ACLB200_VERSION_MAJOR 0
-#define ACLB200_VERSION_MINOR 16
+#define ACLB200_VERSION_MINOR 17
 
 typedef enum aclb200_status
 {
@@ -319,8 +319,10 @@ enum
 	ACLB200_ERROR_FLAG_NEGATIVE_SCALE = 1,		/* informational: a negative scale took rtm::qvv_mul through its matrix branch (qvvf.h:320-345) somewhere */
 	ACLB200_ERROR_FLAG_INVALID_SKELETON = 2,	/* a parent index does not precede its child (the reference reads an unwritten transform there):
 												 * the bone was treated as a root */
-	ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE = 4		/* aclb200_extract_root_motion: a request crossed a loop boundary of a clip compressed with the
+	ACLB200_ERROR_FLAG_WRAP_CLIP_CYCLE = 4,		/* aclb200_extract_root_motion: a request crossed a loop boundary of a clip compressed with the
 												 * wrap policy, whose motion from its last sample back to its first is missing (see there) */
+	ACLB200_ERROR_FLAG_INVALID_MIRROR = 8		/* the mirror decodes and aclb200_mirror_poses: a mirror table entry names a row out of range or a
+												 * row that does not name it back; that row took its own transform (see aclb200_mirror_entry) */
 };
 
 /* One clip to measure == one `calculate_compression_error(allocator, raw_tracks, context, error_metric)` call of the reference
@@ -949,6 +951,100 @@ ACLB200_API aclb200_status aclb200_decompress_tracks_inertialized(aclb200_contex
 ACLB200_API aclb200_status aclb200_decompress_tracks_inertialized_skinning(aclb200_context* context, const aclb200_clipset* clipset,
 	const aclb200_inertialized_request* d_requests, uint32_t num_requests, const aclb200_options* options,
 	const void* d_records, uint64_t num_records, uint64_t record_stride_bytes,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* Mirroring: playing a clip left/right mirrored, so that a motion matching database holds each clip twice (as recorded and mirrored)
+ * while only the recorded copy is authored and compressed. Each row of the mirrored pose takes the transform of its mirror row (left
+ * hand from right hand), reflected across a plane through the origin and corrected for the difference between the two bones' frames.
+ *
+ * Notation as for inertialization: quat_mul(a, b) is rtm's (apply a, then b: the Hamilton product b a), quat_mul_vector3(v, q) is rtm's
+ * (v rotated by q). Every operation is IEEE and unfused; the results equal the reference's rtm::quat_mul and quat_mul_vector3 on any CPU.
+ *
+ * The mirror axis, the normal of the mirror plane: ACLB200_MIRROR_X, _Y or _Z.
+ *   reflect_q(q)   flips the sign bits of the two quaternion vector lanes other than `axis` (X: (x, -y, -z, w))
+ *   reflect_t(t)   flips the sign bit of lane `axis` of the translation (X: (-x, y, z))
+ * Both are sign flips, not subtractions: +0 and -0 swap and NaN payloads are kept.
+ *
+ * The mirror table: one aclb200_mirror_entry per row, 16 byte aligned, in device memory the caller owns. Row i of a pose of n rows has
+ * the partner m = entry[i].mirror when m < n and entry[m].mirror == i; otherwise its partner is i itself and
+ * ACLB200_ERROR_FLAG_INVALID_MIRROR is raised. Partners therefore always pair up. For row i with partner m:
+ *   rotation      quat_mul(quat_mul(entry[i].pre, reflect_q(q_m)), entry[i].post)
+ *   translation   quat_mul_vector3(reflect_t(t_m), entry[i].post)
+ *   scale         s_m, the bits copied
+ * The w lanes of translation and scale are written as 0 (QVV48). Nothing is normalised, and the quat_muls run for identity corrections too.
+ *
+ * In matrix terms the row is C_frame^-1 S X_m S C_i, with S the reflection, pre = C_i and post = conj(C_frame): C_i is the correction
+ * that takes row i's reflected frame to its own, and the frame is what the row is relative to. One table format serves every kind of row:
+ *   local pose rows     frame = the bone's parent (identity for roots); api.py's mirror_table builds this table from a bind pose
+ *   object rows         frame = identity (post = identity)
+ *   feature rows        (aclb200_extract_pose_features, relative to the root) frame = the root
+ *   root motion rows    pre = C_root, post = conj(C_root)
+ * Scale is copied, which is exact when each correction maps every axis onto plus or minus itself (identity, or a half turn about x, y or
+ * z): the corrections rigs use. Corrections that swap axes under non-uniform scale are the caller's responsibility. */
+#define ACLB200_MIRROR_X 0u
+#define ACLB200_MIRROR_Y 1u
+#define ACLB200_MIRROR_Z 2u
+
+/* One row's mirror table entry: 48 bytes, 16 byte aligned. */
+typedef struct aclb200_mirror_entry
+{
+	float    pre[4];		/* quaternion xyzw applied before the reflected rotation */
+	float    post[4];		/* quaternion xyzw applied after it, and to the translation */
+	uint32_t mirror;		/* the row this row takes its transform from */
+	uint32_t reserved[3];	/* ignored */
+} aclb200_mirror_entry;
+
+/* Mirrors num_poses poses of QVV48 rows already on the device: decodes, blends, layer stacks, pose feature rows (num_rows = K, one pose
+ * per (request, offset)), root motion rows (num_rows = 1). Pose p has num_rows rows at p * pose_stride_bytes in d_poses and d_out
+ * (0 = num_rows * 48); row i takes the table entry d_table[i]. d_mirrored (device uint32[num_poses], optional) says per pose:
+ *   NULL   every pose is mirrored
+ *   0      the pose is copied unchanged
+ *   1      the pose is mirrored
+ *   other  the pose is not written
+ * d_out may be d_poses. d_out_flags: device uint32, optional: cleared, then ACLB200_ERROR_FLAG_INVALID_MIRROR OR-ed in when a mirrored
+ * pose met an entry without a partner.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: an unknown axis; NULL or misaligned (16 byte) poses or table, or a
+ * misaligned (4 byte) d_mirrored, with num_poses and num_rows above 0; a pose stride below num_rows * 48 or not a multiple of 16. */
+ACLB200_API aclb200_status aclb200_mirror_poses(aclb200_context* context, const void* d_poses, void* d_out, uint64_t num_poses, uint32_t num_rows,
+	uint64_t pose_stride_bytes, const uint32_t* d_mirrored, const aclb200_mirror_entry* d_table, uint32_t axis, uint32_t* d_out_flags,
+	void* stream);
+
+/* One request of the mirrored decode: the pose to decode and whether to mirror it. 12 bytes, 4 byte aligned. */
+typedef struct aclb200_mirrored_request
+{
+	aclb200_request pose;
+	uint32_t        mirrored;
+} aclb200_mirrored_request;
+
+/* The decode and the mirror in one launch: request r is decoded as aclb200_decompress_tracks decodes its pose; when mirrored == 1 the
+ * rows are then mirrored in shared memory exactly as aclb200_mirror_poses mirrors them (QVV48 and QVV40 rows). Clip c's table starts at
+ * d_mirror_table + d_skeleton_offsets[c] (0 when d_skeleton_offsets is NULL): it is indexed like the parents, so a mirror table belongs to
+ * a skeleton. With parents (d_parent_indices, d_skeleton_offsets and object_kind as aclb200_decompress_tracks_blend) the pose is then
+ * taken to object space, as qvvf or 3x4 matrix rows, by the walk of aclb200_local_to_object_space; without them the rows stay local, in
+ * options->output_layout.
+ *   mirrored == 0                          the rows are byte for byte those of aclb200_decompress_tracks (no parents),
+ *                                          aclb200_decompress_tracks_object_space or _skinning for the same request and options
+ *   mirrored == 1                          the rows are byte for byte aclb200_mirror_poses of the decoded local pose, then the walk and
+ *                                          skinning of aclb200_local_to_object_space or aclb200_local_to_skinning
+ *   any other value, invalid clip          nothing is written for the request, and it is not sought
+ * d_out_flags as the object space decode, plus ACLB200_ERROR_FLAG_INVALID_MIRROR. ACLB200_MATH_FAST is accepted and runs the exact
+ * decode, as in every composed mode.
+ * Refused with ACLB200_ERR_INVALID_ARGUMENT, launching nothing: the refusals of aclb200_decompress_tracks_inertialized (skip masks, a
+ * `skipped` default mode, a scalar clip set, alignment, an unknown object_kind, QVV40 with parents, NULL requests or output with a count
+ * above 0), an unknown axis, a NULL or misaligned (16 byte) table with num_requests > 0. ACLB200_ERR_UNSUPPORTED when one pose does not fit
+ * in a block's shared memory. */
+ACLB200_API aclb200_status aclb200_decompress_tracks_mirrored(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const aclb200_mirror_entry* d_mirror_table, uint32_t axis,
+	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, uint32_t object_kind,
+	void* d_out, uint32_t* d_out_flags, void* stream);
+
+/* The skinning rows of the mirrored pose: aclb200_decompress_tracks_mirrored through the matrix walk and the skinning step of
+ * aclb200_decompress_tracks_skinning (parents and inverse binds required). */
+ACLB200_API aclb200_status aclb200_decompress_tracks_mirrored_skinning(aclb200_context* context, const aclb200_clipset* clipset,
+	const aclb200_mirrored_request* d_requests, uint32_t num_requests, const aclb200_options* options,
+	const aclb200_mirror_entry* d_mirror_table, uint32_t axis,
 	const uint32_t* d_parent_indices, const uint32_t* d_skeleton_offsets, const float* d_inverse_bind,
 	void* d_out, uint32_t* d_out_flags, void* stream);
 
